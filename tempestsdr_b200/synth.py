@@ -47,10 +47,13 @@ def noise_iq(n_pairs: int, seed: int = 0, scale: float = 1.0) -> np.ndarray:
     return (rng.standard_normal(2 * n_pairs) * scale).astype(np.float32)
 
 
-def video_like_frame(w: int, h: int, seed: int = 0, shift_x: int = 0, shift_y: int = 0, noise: float = 0.02) -> np.ndarray:
-    """A w x h float32 frame (already at pixel rate) with blanking strips, circularly shifted."""
+def video_like_frame(w: int, h: int, seed: int = 0, shift_x: int = 0, shift_y: int = 0, noise: float = 0.02,
+                     blank_frac_x: float = 0.14, blank_frac_y: float = 0.05) -> np.ndarray:
+    """A w x h float32 frame (already at pixel rate) with blanking strips, circularly shifted.  The blanking strips take
+    blank_frac_x of the columns and blank_frac_y of the rows (1.0 - 0.14 == 0.86 exactly: the defaults give the frames
+    the golden vectors were made from)."""
     rng = np.random.default_rng(seed)
-    act_w, act_h = int(w * 0.86), int(h * 0.95)
+    act_w, act_h = int(w * (1.0 - blank_frac_x)), int(h * (1.0 - blank_frac_y))
     f = np.full((h, w), 0.05, dtype=np.float32)
     ty, tx = (act_h + 7) // 8, (act_w + 7) // 8
     tiles = rng.uniform(0.35, 1.0, size=(ty, tx)).astype(np.float32)

@@ -151,10 +151,11 @@ def test_pipeline_pll_writeback(items):
     p.close()
 
 
-@pytest.mark.parametrize("name,nframes,batch", [("cfg2", 7, 2), ("cfg5", 3, 1)])
+@pytest.mark.parametrize("name,nframes,batch", [("cfg2", 7, 2), ("cfg5", 3, 1), ("cfg1", 64, 16)])
 def test_pipeline_at_baseline_shapes(name, nframes, batch):
-    """The streaming pipeline at BASELINE's own shapes -- cfg2: 25 MS/s -> 740x1125 frames, cfg5: 50 MS/s -> 1481x1125 -- fed in
-    the RawFile plugin's block size (524 288 floats): frames bit-exact against the stage-wise replay of the reference."""
+    """The streaming pipeline at BASELINE's own shapes -- cfg2: 25 MS/s -> 740x1125 frames, cfg5: 50 MS/s -> 1481x1125, cfg1:
+    8 MS/s -> 507x525 at the e2e benchmark's batch_frames=16, three batches -- fed in the RawFile plugin's block size (524 288
+    floats): frames bit-exact against the stage-wise replay of the reference."""
     from tempestsdr_b200 import pipeline
     from tests.test_gpu_parity import CFGS
     O = orc.best()
@@ -163,7 +164,8 @@ def test_pipeline_at_baseline_shapes(name, nframes, batch):
     items = 512 * 1024
     pairs = (nframes * int(fs / fv) + 3 * int(0.1 * fs / fv))
     nblk = (2 * pairs + items - 1) // items
-    iq_all = synth.video_like_iq(nblk * items // 2, fs, 2576, 1125, fv, seed=73, snr_db=25.0)
+    raster = (800, 525) if name == "cfg1" else (2576, 1125)          # bench.py's raster per shape
+    iq_all = synth.video_like_iq(nblk * items // 2, fs, *raster, fv, seed=73, snr_db=25.0)
     blocks = [iq_all[k * items:(k + 1) * items] for k in range(nblk)]
     _, want = run_oracle_stream(O, blocks, fs, h, fv)
     got = []
@@ -173,7 +175,7 @@ def test_pipeline_at_baseline_shapes(name, nframes, batch):
     for b in blocks:
         p.process(b.copy(), 0)
     p.flush()
-    assert nframes - 1 - batch <= len(got) <= len(want) and len(got) % batch == 0
+    assert nframes - 1 - batch <= len(got) <= len(want) and len(got) % batch == 0      # cfg1: 64 - 17 -> three batches of 16
     for k, (g, ww, hh) in enumerate(got):
         assert (ww, hh) == (w, h) and np.array_equal(g.view(np.uint32), want[k].view(np.uint32)), f"{name} frame {k}"
     p.close()
