@@ -12,7 +12,8 @@
 //   scale, |.|), the ones between through XOR-swizzled shared memory.  Bundling makes every global access a run of >= C
 //   consecutive complex values even on the strided passes, so each pass is one coalesced read + one coalesced write of
 //   the array: 16 N bytes per pass.  The transposing last pass writes to the other buffer, so no copy pass exists.
-//   Real->complex widening and |X|/N are fused into the first / last pass of the autocorrelation's forward transform;
+//   Real->complex widening and |X|/N are fused into the first / last pass of the autocorrelation's forward transform (the
+//   N-point path; on the default half-size path the forward finish is fused into the inverse's first pass, see RSPLIT);
 //   a FAN variant of the last pass stores into the gather buffers of all ranks (superbandwidth, one hop per GPU).
 // Numerics: float32 data.  Layer twiddles come from host-built double-precision tables that carry the REFERENCE'S stage
 // angles (its half-angle recurrence, fft.c:161, is off by up to 5e-5 relative at the largest stages: see
@@ -39,13 +40,17 @@ struct FftPass {
 	long long out_hi, out_lo, out_cs, out_ks;
 	unsigned long long tw_M; long long tw_lo, tw_cs;    // column index = g_lo*tw_lo + c*tw_cs ; tw_M == 0: none
 	float scale;
-	int in_real, out_abs;                               // in_real: 1 = real input widened to (x, 0); 2 = complex input given as PAIRS OF FLOATS that are only 4-byte aligned (in_bs then counts floats)
+	int in_real, out_abs;                               // in_real: 1 = real input widened to (x, 0); 2 = complex input given as PAIRS OF FLOATS that are only 4-byte aligned (in_bs then counts floats); 3 = see rs_* below
 	const float2 *tw_step;                              // host-built W_M^(col (L/8) j), [col][8]; NULL: compute every twiddle
 	float2 *fan[16]; int nfan;                          // FAN kernels: the last stage stores to every fan[p] + offset instead of `out`
 	int exact0;                                         // the first three layers of this pass have eps = 0: plain DFT-8
 	int conj_in, conj_out;                              // inverse transforms: conjugate on load (first pass) / on store (last pass)
 	float *abs_real;                                    // with out_abs: |.| goes here as float32 (same element index) instead of (|.|, 0) to `out` -- may be peer memory
 	int dbg;                                            // timing experiments only (TSDRGPU_FFT_DBG): 1 = no global loads, 2 = no global stores; results are garbage
+	// in_real = 3 (first pass, fft_pass_kernel<..., RSPLIT = true>): `in` is the unscaled half-size forward spectrum Z of a real
+	// sequence (rs_half points per transform) and the input is formed on load as z'[n] = (R[2n], R[2n+1]), R = |X| * rs_scale
+	// from the real split with the last-stage table rs_last (see real_split_rn)
+	const float2 *rs_last; unsigned rs_half; float rs_scale;
 };
 
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
@@ -197,7 +202,23 @@ __device__ __forceinline__ void fft_bulk_g2s(unsigned dst_smem, const void *src,
 	             :: "r"(dst_smem), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-template <int LOG2L, bool FAN = false, bool TMA = false>
+// ---- real-input transforms at half size (see autocorrelation_batch_half) -------------------------------------------------
+// z[j] = x[2j] + i x[2j+1] has been transformed (N/2 points, unscaled) into Z.  With E, O the transforms of the even and odd
+// samples, E = (Z[k] + conj Z[-k]) / 2, O = (Z[k] - conj Z[-k]) / 2i, and the reference's LAST radix-2 stage (its perturbed
+// angle: last[k] = exp(-i pi k / (N/2) (1 + eps_{m-1})), host-built) gives X[k] = E + w O, X[k + N/2] = E - w O with w = last[k]
+// (forward) or conj(last[k]) (inverse).  Explicitly rounded, so that the result does not depend on where it is inlined: the
+// halving is one product on the O side and fused into the final sums on the E side, t = w O is one product and one fused
+// multiply-add per component.
+__device__ __forceinline__ void real_split_rn(float2 zk, float2 zm, float2 w, float2 &x0, float2 &x1) {
+	const float sx = __fadd_rn(zk.x, zm.x), dy = __fsub_rn(zk.y, zm.y);
+	const float ox = __fmul_rn(__fadd_rn(zk.y, zm.y), 0.5f), oy = __fmul_rn(__fsub_rn(zk.x, zm.x), -0.5f);
+	const float tx = __fmaf_rn(w.x, ox, -__fmul_rn(w.y, oy)), ty = __fmaf_rn(w.x, oy, __fmul_rn(w.y, ox));
+	x0 = make_float2(__fmaf_rn(sx, 0.5f, tx), __fmaf_rn(dy, 0.5f, ty));
+	x1 = make_float2(__fmaf_rn(sx, 0.5f, -tx), __fmaf_rn(dy, 0.5f, -ty));
+}
+
+// RSPLIT: the first pass of the inverse half-size transform (FftPass.in_real = 3) -- the forward finish happens on load
+template <int LOG2L, bool FAN = false, bool TMA = false, bool RSPLIT = false>
 __global__ void __launch_bounds__(512, 3) fft_pass_kernel(const float2 *in, float2 *out, FftPass P, const float2 *__restrict__ stw) {
 	extern __shared__ __align__(128) float2 s[];
 	constexpr int L = 1 << LOG2L, NST8 = LOG2L / 3, RL = LOG2L % 3;
@@ -252,7 +273,30 @@ __global__ void __launch_bounds__(512, 3) fft_pass_kernel(const float2 *in, floa
 			}
 		} else if (active) {
 			const int off = c * (int) P.in_cs + i * (int) P.in_js, step = L8 * (int) P.in_js;
-			if (P.in_real == 2) {                             // pairs of floats, 4-byte aligned (a capture that starts on an odd sample)
+			if (RSPLIT) {
+				// v[m] = z'[n] and v[m + 4] = z'[n + M/2] (n = n0 + m step, 4 step = M/2 in every plan) come from the same two splits,
+				// at K = 2n and 2n + 1: R[K] = |x0| and R[K + M] = |x1|.  Z[2n], Z[2n+1] and last[2n], last[2n+1] are one 16-byte
+				// load each; the mirrors Z[M - 2n], Z[M - 2n - 1] of adjacent columns are a contiguous run read backwards.
+				const unsigned M = P.rs_half;
+				const float2 *z = in + (long long) blockIdx.y * P.in_bs;
+				const unsigned n0 = (unsigned) (in_base - (long long) blockIdx.y * P.in_bs) + (unsigned) off;
+				#pragma unroll
+				for (int m = 0; m < 4; m++) {
+					const unsigned K = 2u * (n0 + (unsigned) (m * step));
+					const float4 zk = __ldg(reinterpret_cast<const float4 *>(z + K)), w = __ldg(reinterpret_cast<const float4 *>(P.rs_last + K));
+					const float2 zm0 = __ldg(z + ((M - K) & (M - 1))), zm1 = __ldg(z + (M - K - 1));
+					float2 a0, a1, b0, b1;
+					real_split_rn(make_float2(zk.x, zk.y), zm0, make_float2(w.x, w.y), a0, a1);
+					real_split_rn(make_float2(zk.z, zk.w), zm1, make_float2(w.z, w.w), b0, b1);
+					const float s = P.rs_scale;
+					v[m] = make_float2(mag_exact(__fmul_rn(a0.x, s), __fmul_rn(a0.y, s)), mag_exact(__fmul_rn(b0.x, s), __fmul_rn(b0.y, s)));
+					v[m + 4] = make_float2(mag_exact(__fmul_rn(a1.x, s), __fmul_rn(a1.y, s)), mag_exact(__fmul_rn(b1.x, s), __fmul_rn(b1.y, s)));
+				}
+				if (P.conj_in) {
+					#pragma unroll
+					for (int m = 0; m < 8; m++) v[m].y = -v[m].y;
+				}
+			} else if (P.in_real == 2) {                             // pairs of floats, 4-byte aligned (a capture that starts on an odd sample)
 				const float *gr = reinterpret_cast<const float *>(in) + (long long) blockIdx.y * P.in_bs + 2 * (in_base + off);
 				#pragma unroll
 				for (int m = 0; m < 8; m++) v[m] = make_float2(__ldg(gr + 2 * m * step), __ldg(gr + 2 * m * step + 1));
@@ -410,29 +454,8 @@ __global__ void k_abs(float2 *answer, unsigned long long from, unsigned long lon
 		answer[i] = make_float2(mag_exact(v.x, v.y), 0.0f);
 	}
 }
-// ---- real-input transforms at half size (opt-in, see autocorrelation_batch) ------------------------------------------------
-// z[j] = x[2j] + i x[2j+1] has been transformed (N/2 points, unscaled) into Z.  With E, O the transforms of the even and odd
-// samples, E = (Z[k] + conj Z[-k]) / 2, O = (Z[k] - conj Z[-k]) / 2i, and the reference's LAST radix-2 stage (its perturbed
-// angle: last[k] = exp(-i pi k / (N/2) (1 + eps_{m-1})), host-built) gives X[k] = E + last[k] O, X[k + N/2] = E - last[k] O.
-__device__ __forceinline__ void real_split(float2 zk, float2 zm, float2 w, float2 &x0, float2 &x1) {
-	const float2 e = make_float2(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
-	const float2 o = make_float2(0.5f * (zk.y + zm.y), -0.5f * (zk.x - zm.x));
-	const float2 t = make_float2(w.x * o.x - w.y * o.y, w.x * o.y + w.y * o.x);
-	x0 = make_float2(e.x + t.x, e.y + t.y); x1 = make_float2(e.x - t.x, e.y - t.y);
-}
-// forward: R[k] = |X[k]| / N for all N outputs, as REAL numbers (they are the next transform's real input); grid.y = batch
-__global__ void __launch_bounds__(256) k_real_fwd_finish(const float2 *__restrict__ Z, long long z_bs, const float2 *__restrict__ last,
-                                                         unsigned half, float inv_n, float *__restrict__ R, long long r_bs) {
-	const float2 *z = Z + (long long) blockIdx.y * z_bs;
-	float *r = R + (long long) blockIdx.y * r_bs;
-	for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < half; k += gridDim.x * blockDim.x) {
-		float2 x0, x1;
-		real_split(z[k], z[(half - k) & (half - 1)], __ldg(last + k), x0, x1);
-		r[k] = mag_exact(x0.x * inv_n, x0.y * inv_n);
-		r[k + half] = mag_exact(x1.x * inv_n, x1.y * inv_n);
-	}
-}
-// inverse (no scaling, conjugate twiddle): the N complex outputs
+// ---- the inverse half-size transform's finish (real_split_rn): every one of the N complex outputs of an autocorrelation, for
+// callers that want all lags (the frame-rate detector folds the lags it reads into its running means, k_accumulate_half)
 __global__ void __launch_bounds__(256) k_real_inv_finish(const float2 *__restrict__ Z, long long z_bs, const float2 *__restrict__ last,
                                                          unsigned half, float2 *__restrict__ Y, long long y_bs) {
 	const float2 *z = Z + (long long) blockIdx.y * z_bs;
@@ -440,24 +463,8 @@ __global__ void __launch_bounds__(256) k_real_inv_finish(const float2 *__restric
 	for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < half; k += gridDim.x * blockDim.x) {
 		const float2 w = __ldg(last + k);
 		float2 x0, x1;
-		real_split(z[k], z[(half - k) & (half - 1)], make_float2(w.x, -w.y), x0, x1);
+		real_split_rn(z[k], z[(half - k) & (half - 1)], make_float2(w.x, -w.y), x0, x1);
 		y[k] = x0; y[k + half] = x1;
-	}
-}
-
-// the same, but only the lags a caller will read: lags [lo0, hi0) and [lo1, hi1), all below `half` (the frame-rate detector's
-// two windows, frameratedetector.c:91-95): the kernel touches (hi0-lo0)+(hi1-lo1) lags instead of N
-__global__ void __launch_bounds__(256) k_real_inv_finish_win(const float2 *__restrict__ Z, long long z_bs, const float2 *__restrict__ last,
-                                                             unsigned half, float2 *__restrict__ Y, long long y_bs, unsigned lo0, unsigned hi0, unsigned lo1, unsigned hi1) {
-	const float2 *z = Z + (long long) blockIdx.y * z_bs;
-	float2 *y = Y + (long long) blockIdx.y * y_bs;
-	const unsigned n0 = hi0 - lo0, total = n0 + (hi1 - lo1);
-	for (unsigned t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
-		const unsigned k = (t < n0) ? (lo0 + t) : (lo1 + (t - n0));
-		const float2 w = __ldg(last + k);
-		float2 x0, x1;
-		real_split(z[k], z[(half - k) & (half - 1)], make_float2(w.x, -w.y), x0, x1);
-		y[k] = x0;
 	}
 }
 
@@ -487,6 +494,27 @@ __global__ void k_accumulate_batch(double *out, unsigned long long first_calls, 
 			const unsigned long long calls = first_calls + b;
 			const float2 v = in[(size_t) b * in_stride + startid + i];
 			const double re = (double) v.x, im = (double) v.y;
+			const double mag = __dsqrt_rn(__dadd_rn(__dmul_rn(re, re), __dmul_rn(im, im)));
+			acc = (calls == 0) ? mag : __ddiv_rn(__dadd_rn(__dmul_rn(acc, (double) (calls - 1)), mag), (double) calls);
+		}
+		out[i] = acc;
+	}
+}
+// the same, straight from the half-size inverse's output Z' (captures z_bs apart, `half` points each): the inverse finish is
+// folded in, lag k < half is x0 of the split at k, lag k >= half (a window beyond N/2) x1 of the split at k - half, both with
+// the conjugate last-stage twiddle, exactly as k_real_inv_finish forms them
+__global__ void k_accumulate_half(double *out, unsigned long long first_calls, const float2 *__restrict__ Z, long long z_bs, unsigned batch,
+                                  const float2 *__restrict__ last, unsigned half, int startid, int length) {
+	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < length; i += gridDim.x * blockDim.x) {
+		const unsigned k = (unsigned) (startid + i), hi = k >= half, kk = hi ? k - half : k, km = (half - kk) & (half - 1);
+		const float2 w = __ldg(last + kk), wc = make_float2(w.x, -w.y);
+		double acc = out[i];
+		for (unsigned b = 0; b < batch; b++) {
+			const unsigned long long calls = first_calls + b;
+			const float2 *z = Z + (long long) b * z_bs;
+			float2 x0, x1;
+			real_split_rn(z[kk], z[km], wc, x0, x1);
+			const double re = (double) (hi ? x1.x : x0.x), im = (double) (hi ? x1.y : x0.y);
 			const double mag = __dsqrt_rn(__dadd_rn(__dmul_rn(re, re), __dmul_rn(im, im)));
 			acc = (calls == 0) ? mag : __ddiv_rn(__dadd_rn(__dmul_rn(acc, (double) (calls - 1)), mag), (double) calls);
 		}
@@ -683,7 +711,8 @@ int ensure_table(tsdrgpu_ctx_t *ctx, cudaStream_t stream) {
 	const int max_smem = (int) (2 * sizeof(float2) * FFT_MAX_ELEMS);     // ping-pong
 #define SET_ATTR(l) CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
 	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
-	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem))
+	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
+	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem))
 	SET_ATTR(3); SET_ATTR(4); SET_ATTR(5); SET_ATTR(6); SET_ATTR(7); SET_ATTR(8); SET_ATTR(9); SET_ATTR(10); SET_ATTR(11);
 #undef SET_ATTR
 	g_attr_set[ctx->device] = true;
@@ -712,6 +741,7 @@ int launch_pass(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float
 	const int nstages = P.log2L / 3 + ((P.log2L % 3) ? 1 : 0);
 	const dim3 grid(bundles, batch);
 	if (P.log2L <= 2) {
+		if (P.in_real == 3) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "real-split input needs lines of >= 8 points", cudaSuccess, __FILE__, __LINE__);
 		if (P.log2L == 1) KL(ctx, "fft_pass_kernel", stream, fft_tiny_kernel<1><<<dim3(1, batch), 32, 0, stream>>>(in, out, P));
 		else KL(ctx, "fft_pass_kernel", stream, fft_tiny_kernel<2><<<dim3(1, batch), 32, 0, stream>>>(in, out, P));
 		return TSDRGPU_OK;
@@ -734,6 +764,7 @@ int launch_pass(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float
 	const size_t smem = sizeof(float2) * (size_t) total * ((nstages >= 3 || (tma && nstages == 2)) ? 2 : 1);
 	switch (P.log2L) {
 #define CASE(l) case l: if (P.nfan > 0) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, true, false><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
+	                else if (P.in_real == 3) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, false, true><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
 	                else if (tma) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, true><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
 	                else KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, false><<<grid, threads, smem, stream>>>(in, out, P, stw)); break
 	CASE(3); CASE(4); CASE(5); CASE(6); CASE(7); CASE(8); CASE(9); CASE(10); CASE(11);
@@ -751,18 +782,21 @@ struct FftOpts {
 	const float2 *cplx_in; long long cplx_bs; // the first pass reads its (complex) input from here instead of `data` (which is then output only)
 	const float *pair_in; long long pair_bs;  // the same, but the input is pairs of floats with 4-byte alignment only; pair_bs in FLOATS
 	float *abs_real;                          // with out_abs (batch 1): the final pass stores |.| as float32 here (peer memory allowed) and leaves `data` alone
+	const float2 *split_in; long long split_bs;   // the first pass forms its input from this half-size spectrum (FftPass.in_real = 3); must not be `scratch`,
+	const float2 *split_last; float split_scale;  // nor `data` on one-pass plans
 };
 
 // N-point transform of `data` (complex, natural order) through `scratch`; result lands in `data`.
 // With opts.real_in the input is read from a real array instead (data is output only).
 int fft_run(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, float2 *scratch, unsigned log2N, int inverse, FftOpts o) {
 	const unsigned long long N = 1ull << log2N;
-	const float2 *src0 = o.real_in ? reinterpret_cast<const float2 *>(o.real_in) : (o.pair_in ? reinterpret_cast<const float2 *>(o.pair_in) : (o.cplx_in ? o.cplx_in : data));
-	const long long in0_bs = o.real_in ? o.real_bs : (o.pair_in ? o.pair_bs : (o.cplx_in ? o.cplx_bs : o.data_bs));
-	const int in_mode = o.real_in ? 1 : (o.pair_in ? 2 : 0);
+	const float2 *src0 = o.split_in ? o.split_in : (o.real_in ? reinterpret_cast<const float2 *>(o.real_in) : (o.pair_in ? reinterpret_cast<const float2 *>(o.pair_in) : (o.cplx_in ? o.cplx_in : data)));
+	const long long in0_bs = o.split_in ? o.split_bs : (o.real_in ? o.real_bs : (o.pair_in ? o.pair_bs : (o.cplx_in ? o.cplx_bs : o.data_bs)));
+	const int in_mode = o.split_in ? 3 : (o.real_in ? 1 : (o.pair_in ? 2 : 0));
 	double eps_all[40];
 	tsdrgpu_fft_reference_eps((int) log2N < 40 ? (int) log2N : 40, inverse, eps_all);
 	FftPass P; memset(&P, 0, sizeof P);
+	P.rs_last = o.split_last; P.rs_half = (unsigned) N; P.rs_scale = o.split_scale;     // (read by the first pass only, with in_real = 3)
 	auto with_fan = [&](FftPass &F) {                   // the pass that produces the final result
 		F.nfan = 0;
 		if (o.fan && o.nfan > 0 && !inverse) { F.nfan = o.nfan < 16 ? o.nfan : 16; for (int q = 0; q < F.nfan; q++) F.fan[q] = o.fan[q]; }
@@ -900,7 +934,7 @@ int tsdrgpu_argmax_mag_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const f
 
 struct tsdrgpu_frd {
 	tsdrgpu_ctx_t *ctx;
-	float *d_big; size_t big_cap;                 // extbuff (2*size floats)
+	float *d_big; size_t big_cap;                 // extbuff (2*size floats), only where the answers are materialised (see frd_run_impl)
 	double *d_p1, *d_p2; size_t p1_cap, p2_cap;   // the two running means
 	uint64_t calls; int fresh;
 	int *d_peaks;                                 // first strict maximum of each plot (k_plot_peaks), refreshed with every run
@@ -948,12 +982,14 @@ static int last_stage_table(tsdrgpu_ctx_t *ctx, unsigned half, double eps, const
 	return TSDRGPU_OK;
 }
 
-// Default path (TSDRGPU_AUTOCORR_FULL=1 opts out): both transforms of the
-// autocorrelation at half size.  The capture and |X|/N are
-// real; a real sequence of length N is a complex one of length N/2, one N/2-point transform + the reference's last radix-2
-// stage (k_real_*_finish) gives the N-point result.  profiles/studies/real_input_autocorr_study.py measures the only
-// approximation (the mirror identity under perturbed stage angles): 6.6e-10 of the zero-lag peak at 2^20, 7.9e-9 at 2^22.
-struct LagWindows { unsigned lo0, hi0, lo1, hi1; };      // only these lags of every answer are needed (all zero: every lag)
+// Default path (TSDRGPU_AUTOCORR_FULL=1 opts out): both transforms of the autocorrelation at half size.  The capture and |X|/N
+// are real; a real sequence of length N is a complex one of length N/2, one N/2-point transform + the reference's last radix-2
+// stage (real_split_rn) gives the N-point result.  Neither finish is a pass of its own: the forward's is formed by the inverse's
+// first pass as it loads (FftPass.in_real = 3), the inverse's by k_real_inv_finish for callers that want every lag or by
+// k_accumulate_half for the frame-rate detector, which only reads its two windows.  profiles/studies/real_input_autocorr_study.py
+// measures the only approximation (the mirror identity under perturbed stage angles): 6.6e-10 of the zero-lag peak at 2^20,
+// 7.9e-9 at 2^22.
+static bool autocorr_half_size(unsigned long long N) { return N >= 16 && getenv("TSDRGPU_AUTOCORR_FULL") == NULL; }     // read per call: the tests flip it inside one process
 
 // How many captures share one pair of work buffers (TSDRGPU_AUTOCORR_GROUP; default: the whole batch).  Small groups would keep
 // the intermediates of the four passes inside the L2 instead of streaming them through HBM, but the pass kernel is bound by
@@ -966,9 +1002,14 @@ static unsigned autocorr_group(unsigned long long N, unsigned batch) {
 	return batch;
 }
 
+// the frame-rate detector's two running means (frameratedetector.c:34-62): lags [start1, start1 + len1) into p1, [start2, ...)
+// into p2, all below N; the first capture of the batch is call number first_calls
+struct RunningMeans { double *p1, *p2; int start1, len1, start2, len2; unsigned long long first_calls; };
+
 struct WorkBufs { float2 *w0, *w1; };                     // caller-owned work buffers (NULL: the context's scratch slots 0 and 1)
+// every lag of every capture into ans (rm == NULL), or only the lags of the running means, folded into them (rm != NULL; ans unused)
 static int autocorrelation_batch_half(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *ans, long long ans_bs, const float *d_real,
-                                      long long real_stride, unsigned long long N, unsigned batch, LagWindows win, WorkBufs wb) {
+                                      long long real_stride, unsigned long long N, unsigned batch, const RunningMeans *rm, WorkBufs wb) {
 	const unsigned log2N = ilog2(N), half = (unsigned) (N >> 1);
 	double eps_all[40];
 	tsdrgpu_fft_reference_eps((int) log2N, 0, eps_all);
@@ -981,10 +1022,11 @@ static int autocorrelation_batch_half(tsdrgpu_ctx_t *ctx, cudaStream_t stream, f
 	if (!w0_ && (rc = tsdrgpu_scratch(ctx, 0, sizeof(float2) * half * G, &w0_))) return rc;
 	if (!w1_ && (rc = tsdrgpu_scratch(ctx, 1, sizeof(float2) * half * G, &w1_))) return rc;
 	float2 *W0 = (float2 *) w0_, *W1 = (float2 *) w1_;
-	const bool windowed = win.hi0 > win.lo0 || win.hi1 > win.lo1;
+	// the inverse's first pass reads Z (in W1) while other CTAs write: to the scratch W0 on multi-pass plans (Z' then lands in
+	// W1), to its output on one-pass plans (Z' lands in W0)
+	float2 *Zi = (log2N - 1 <= (unsigned) FFT_MAX_LOG2L) ? W0 : W1;
 	for (unsigned g0 = 0; g0 < batch; g0 += G) {
 		const unsigned gb = (batch - g0 < G) ? (batch - g0) : G;
-		const dim3 grid(grid1d(half, ctx->sm_count), gb);
 		// forward: Z = FFT_{N/2}(capture viewed as complex pairs), unscaled: capture -> W0 -> W1
 		FftOpts f; memset(&f, 0, sizeof f);
 		f.scale = 1.0f; f.batch = gb; f.data_bs = (long long) half; f.scratch_bs = (long long) half;
@@ -992,25 +1034,24 @@ static int autocorrelation_batch_half(tsdrgpu_ctx_t *ctx, cudaStream_t stream, f
 		if ((real_stride & 1) || (reinterpret_cast<unsigned long long>(cap0) & 7ull)) { f.pair_in = cap0; f.pair_bs = real_stride; }   // odd capture sizes: every other capture starts on an odd sample
 		else { f.cplx_in = reinterpret_cast<const float2 *>(cap0); f.cplx_bs = real_stride / 2; }
 		if ((rc = fft_run(ctx, stream, W1, W0, log2N - 1, 0, f))) return rc;
-		// R = |X| / N as N reals = N/2 complex: W1 -> W0
-		KL(ctx, "k_real_fwd_finish", stream, k_real_fwd_finish<<<grid, 256, 0, stream>>>(W1, (long long) half, last, half, 1.0f / (float) N,
-		                                                                                  reinterpret_cast<float *>(W0), (long long) N));
-		// inverse: Z' = IFFT_{N/2}(R viewed as complex pairs): W0 -> W1 -> W0
+		// inverse: Z' = IFFT_{N/2}(z'), z'[n] = (R[2n], R[2n+1]) with R = |X| / N formed from Z on load
 		FftOpts gopt; memset(&gopt, 0, sizeof gopt);
 		gopt.scale = 1.0f; gopt.batch = gb; gopt.data_bs = (long long) half; gopt.scratch_bs = (long long) half;
-		if ((rc = fft_run(ctx, stream, W0, W1, log2N - 1, 1, gopt))) return rc;
-		float2 *out = ans + (long long) g0 * ans_bs;
-		if (windowed) {
-			const unsigned total = (win.hi0 - win.lo0) + (win.hi1 - win.lo1);
-			KL(ctx, "k_real_inv_finish", stream, k_real_inv_finish_win<<<dim3(grid1d(total, ctx->sm_count), gb), 256, 0, stream>>>(W0, (long long) half, last, half, out, ans_bs,
-				win.lo0, win.hi0, win.lo1, win.hi1));
-		} else KL(ctx, "k_real_inv_finish", stream, k_real_inv_finish<<<grid, 256, 0, stream>>>(W0, (long long) half, last, half, out, ans_bs));
+		gopt.split_in = W1; gopt.split_bs = (long long) half; gopt.split_last = last; gopt.split_scale = 1.0f / (float) N;
+		if ((rc = fft_run(ctx, stream, Zi, W0, log2N - 1, 1, gopt))) return rc;
+		if (rm) {                                      // before the next group reuses the work buffers; captures stay in order
+			if (rm->len1) KL(ctx, "k_accumulate", stream, k_accumulate_half<<<grid1d((unsigned long long) rm->len1, ctx->sm_count), 256, 0, stream>>>(
+				rm->p1, rm->first_calls + g0, Zi, (long long) half, gb, last, half, rm->start1, rm->len1));
+			if (rm->len2) KL(ctx, "k_accumulate", stream, k_accumulate_half<<<grid1d((unsigned long long) rm->len2, ctx->sm_count), 256, 0, stream>>>(
+				rm->p2, rm->first_calls + g0, Zi, (long long) half, gb, last, half, rm->start2, rm->len2));
+		} else KL(ctx, "k_real_inv_finish", stream, k_real_inv_finish<<<dim3(grid1d(half, ctx->sm_count), gb), 256, 0, stream>>>(
+			Zi, (long long) half, last, half, ans + (long long) g0 * ans_bs, ans_bs));
 	}
 	return TSDRGPU_OK;
 }
 
 static int autocorrelation_batch(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float *d_answer, long long answer_stride,
-                                 const float *d_real, long long real_stride, uint32_t size, unsigned batch, bool skip_tail, LagWindows win = LagWindows{0, 0, 0, 0},
+                                 const float *d_real, long long real_stride, uint32_t size, unsigned batch, bool skip_tail,
                                  WorkBufs wb = WorkBufs{NULL, NULL}) {
 	int rc = ensure_table(ctx, stream);
 	if (rc) return rc;
@@ -1027,11 +1068,8 @@ static int autocorrelation_batch(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float 
 		if (N == 1) return TSDRGPU_OK;
 	}
 	// default: both transforms at half size (autocorrelation_batch_half); TSDRGPU_AUTOCORR_FULL=1 keeps the N-point transforms
-	const bool full_size = getenv("TSDRGPU_AUTOCORR_FULL") != NULL;     // read per call: the tests flip it inside one process
-	if (!full_size && N >= 16 && (answer_stride & 1) == 0) {
-		if (win.hi0 > (unsigned) (N >> 1) || win.hi1 > (unsigned) (N >> 1)) win = LagWindows{0, 0, 0, 0};      // a window beyond N/2: produce every lag
-		return autocorrelation_batch_half(ctx, stream, ans, answer_stride / 2, d_real, real_stride, N, batch, win, wb);
-	}
+	if (autocorr_half_size(N) && (answer_stride & 1) == 0)
+		return autocorrelation_batch_half(ctx, stream, ans, answer_stride / 2, d_real, real_stride, N, batch, NULL, wb);
 	void *scratch = wb.w0;                              // (sized for N * batch by the overlapped detector)
 	if (!scratch && (rc = tsdrgpu_scratch(ctx, 0, sizeof(float2) * N * batch, &scratch))) return rc;
 	// forward transform of the first N samples, real input widened on load, |X|/N on store
@@ -1150,7 +1188,9 @@ static int frd_run_impl(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, co
 	const uint32_t N = tsdrgpu_fft_getrealsize(size);
 	ARG_TRY(ctx, (uint64_t) fmax <= (uint64_t) size && flen >= 0 && llen >= 0);
 	const bool skip_tail = (uint32_t) fmax <= N;               // always true for the detector's own capture size
-	const size_t big_need = 2ull * size * batch;
+	// default: the running means are taken straight from the half-size inverse's output, no lag is stored; otherwise (N-point
+	// transforms, or lags beyond the transformed ones) the answers are materialised in d_big and read back
+	const bool fold = skip_tail && autocorr_half_size(N);
 	WorkBufs wb = WorkBufs{NULL, NULL};
 	if (f->overlap) {
 		// the internal stream picks up behind everything the caller's stream holds now (the capture is complete there)
@@ -1168,11 +1208,6 @@ static int frd_run_impl(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, co
 		CU_TRY(ctx, cudaEventRecord(f->ev_in, caller));
 		CU_TRY(ctx, cudaStreamWaitEvent(f->s_side, f->ev_in, 0));
 	}
-	if (f->big_cap < big_need) {
-		CU_TRY(ctx, cudaStreamSynchronize(stream));
-		if (f->d_big) CU_TRY(ctx, cudaFree(f->d_big));
-		CU_TRY(ctx, cudaMalloc(&f->d_big, sizeof(float) * big_need)); f->big_cap = big_need;
-	}
 	if (f->p1_cap < (size_t) flen || f->fresh) {
 		if (f->p1_cap < (size_t) flen) { CU_TRY(ctx, cudaStreamSynchronize(stream)); if (f->d_p1) CU_TRY(ctx, cudaFree(f->d_p1)); CU_TRY(ctx, cudaMalloc(&f->d_p1, sizeof(double) * (flen + 1))); f->p1_cap = flen; }
 		CU_TRY(ctx, cudaMemsetAsync(f->d_p1, 0, sizeof(double) * (flen + 1), stream));
@@ -1185,12 +1220,22 @@ static int frd_run_impl(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, co
 	const uint64_t first_calls = f->calls + 1;                  // extbuffer.c:81, one prepare per capture
 	f->calls += batch;
 	int rc;
-	// only the two lag windows are ever read (frameratedetector.c:106-109): the last step writes nothing else
-	LagWindows win = LagWindows{0, 0, 0, 0};
-	if (skip_tail && !getenv("TSDRGPU_AUTOCORR_ALL_LAGS")) win = LagWindows{(unsigned) fmin, (unsigned) fmax, (unsigned) lmin, (unsigned) lmax};
-	if ((rc = autocorrelation_batch(ctx, stream, f->d_big, 2ll * size, d_capture, (long long) capture_stride, size, batch, skip_tail, win, wb))) return rc;
-	if (flen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) flen, ctx->sm_count), 256, 0, stream>>>(f->d_p1, first_calls, reinterpret_cast<const float2 *>(f->d_big), (long long) size, batch, fmin, flen));
-	if (llen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) llen, ctx->sm_count), 256, 0, stream>>>(f->d_p2, first_calls, reinterpret_cast<const float2 *>(f->d_big), (long long) size, batch, lmin, llen));
+	if (fold) {
+		// only the two lag windows are ever read (frameratedetector.c:106-109)
+		if ((rc = ensure_table(ctx, stream))) return rc;
+		const RunningMeans rm = {f->d_p1, f->d_p2, fmin, flen, lmin, llen, first_calls};
+		if ((rc = autocorrelation_batch_half(ctx, stream, NULL, 0, d_capture, (long long) capture_stride, N, batch, &rm, wb))) return rc;
+	} else {
+		const size_t big_need = 2ull * size * batch;
+		if (f->big_cap < big_need) {
+			CU_TRY(ctx, cudaStreamSynchronize(stream));
+			if (f->d_big) CU_TRY(ctx, cudaFree(f->d_big));
+			CU_TRY(ctx, cudaMalloc(&f->d_big, sizeof(float) * big_need)); f->big_cap = big_need;
+		}
+		if ((rc = autocorrelation_batch(ctx, stream, f->d_big, 2ll * size, d_capture, (long long) capture_stride, size, batch, skip_tail, wb))) return rc;
+		if (flen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) flen, ctx->sm_count), 256, 0, stream>>>(f->d_p1, first_calls, reinterpret_cast<const float2 *>(f->d_big), (long long) size, batch, fmin, flen));
+		if (llen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) llen, ctx->sm_count), 256, 0, stream>>>(f->d_p2, first_calls, reinterpret_cast<const float2 *>(f->d_big), (long long) size, batch, lmin, llen));
+	}
 	KL(ctx, "k_plot_peaks", stream, k_plot_peaks<<<2, 1024, 0, stream>>>(f->d_p1, flen, f->d_p2, llen, f->d_peaks));
 	if (calls) *calls = f->calls;
 	if (h_frame_plot || h_line_plot) {
