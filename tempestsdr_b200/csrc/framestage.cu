@@ -17,13 +17,15 @@
 // single-precision row/column sums are accumulated in exactly the reference's order (one owner thread per
 // row / per column).  Only `snr` (dead in the reference, dsp.c:234) uses tree-ordered double sums.
 //
-// Every other kernel here is HBM-bound elementwise/reduction work: coalesced (vectorised where aligned) loads, cp.async rings
-// for the order-bound row/column sums, grid sized by pixels x frames.
+// Every other kernel here is HBM-bound elementwise/reduction work: coalesced (vectorised where aligned) loads, rings in shared
+// memory (tensor-map or cp.async copies) for the order-bound row/column sums, grid sized by pixels x frames.
 #include "common.cuh"
 #include "host_plan.h"
 #include <math.h>
 #include <stdlib.h>
 #include <cuda_pipeline.h>
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
 
@@ -251,20 +253,112 @@ __global__ void __launch_bounds__(256) fs_norm_lowpass(const float *__restrict__
 
 // ---------------------------------------------------------------- row / column collapse (dsp.c:96-110)
 // Sequential single-precision accumulation in raster order == per column: top to bottom; per row: left to right.
-// grid.x = column CTAs (128 columns each) followed by row CTAs (64 rows each); grid.y = frame.
+// grid.x = column CTAs followed by row CTAs; grid.y = frame.
 // Both sums are chains of dependent additions (1125 per column, 740 per row at cfg2) that may not be re-associated, so
 // the only parallelism is across chains; what has to be hidden is the memory latency inside a chain.  A CTA streams its
-// slab of the frame through a 4-stage ring in shared memory with cp.async (the next three stages are in flight while one
-// is summed), the owner threads read their operands from shared memory:
+// slab of the frame through a ring of stages in shared memory (the next stages are in flight while one is summed), the
+// owner threads read their operands from shared memory.  The frame is read twice; the second read comes from L2 only if it
+// follows the first closely (see fs_collapse_tiles).
+//
+// fs_collapse_tiles: rows on 16-byte boundaries (w % 4 == 0, aligned base).  The ring is filled by 2-D tensor copies
+// (cp.async.bulk.tensor, one request per box of the 3-D tensor map x = column, y = row, z = frame), issued by one thread and
+// counted in bytes on the stage's mbarrier: nobody spends issue slots on copies or their addresses, and every thread owns a chain.
+// A CTA is one warp:
+//   column CTA: 32 columns x all rows, boxes of 32 columns x 64 rows (8 KB, 8 stages), lane c owns column c;
+//   row CTA:    32 rows x all columns, boxes of 32 columns (128 B, 128-byte swizzle) x 32 rows (4 KB, 8 stages), lane r owns row r.
+// Narrow CTAs make many per frame (24 + 36 at cfg2), so the resident ones (3 per SM by shared memory) cover ~7 frames at a time:
+// a column CTA sweeps its frame top to bottom while the row CTAs of that frame run, so less is read in between and more of the
+// second read is served by the L2.
+// With CTAs of 128 columns / 128 rows (15 per frame, ~35 frames open) the second read mostly missed: 0.157 against 0.119 ms per
+// 64-frame cfg2 launch on an H100 SXM at a 400 W power limit (smaller rings, 4 CTAs per SM: 0.121).
+// The tensor map fills what lies beyond the frame's last column / row with zeros; those slots never enter a chain (x + 0.0f is
+// not x when x = -0.0f): the loops are bounded by the columns / rows that exist.
+constexpr int CT_THREADS = 32;
+constexpr int CT_COLS = 32, CT_CROWS = 64, CT_CSTAGES = 8;      // column CTA box: 8 KB
+constexpr int CT_RCOLS = 32, CT_ROWS = 32, CT_RSTAGES = 8;      // row CTA box: 4 KB
+constexpr int CT_RING = CT_CSTAGES * CT_COLS * CT_CROWS * 4 > CT_RSTAGES * CT_RCOLS * CT_ROWS * 4 ? CT_CSTAGES * CT_COLS * CT_CROWS * 4
+                                                                                                  : CT_RSTAGES * CT_RCOLS * CT_ROWS * 4;
+constexpr int CT_SMEM = CT_RING + 1024;                 // + slack to put the ring on the 1024-byte boundary the swizzle repeats on
+
+__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count) : "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory"); }
+__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
+	asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
+	             :: "r"(bar), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void tma_box3(unsigned dst_smem, const CUtensorMap *map, int x, int y, int z, unsigned bar) {
+	asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+	             :: "r"(dst_smem), "l"(reinterpret_cast<unsigned long long>(map)), "r"(x), "r"(y), "r"(z), "r"(bar) : "memory");
+}
+
+__global__ void __launch_bounds__(CT_THREADS) fs_collapse_tiles(const __grid_constant__ CUtensorMap cmap, const __grid_constant__ CUtensorMap rmap,
+                                                                int w, int h, float *__restrict__ wbuf, float *__restrict__ hbuf, int col_ctas) {
+	extern __shared__ unsigned char ct_smem[];
+	__shared__ __align__(8) unsigned long long bars[CT_CSTAGES > CT_RSTAGES ? CT_CSTAGES : CT_RSTAGES];
+	const unsigned raw = (unsigned) __cvta_generic_to_shared(ct_smem), ring_a = (raw + 1023u) & ~1023u;
+	const float *ring = reinterpret_cast<const float *>(ct_smem + (ring_a - raw));
+	const unsigned bar_a = (unsigned) __cvta_generic_to_shared(bars);
+	const int f = blockIdx.y, tid = threadIdx.x;
+	const bool colcta = (int) blockIdx.x < col_ctas;
+	const int stages = colcta ? CT_CSTAGES : CT_RSTAGES;
+	const unsigned box_bytes = colcta ? CT_COLS * CT_CROWS * 4 : CT_RCOLS * CT_ROWS * 4;
+	const int x0 = colcta ? blockIdx.x * CT_COLS : 0, y0 = colcta ? 0 : ((int) blockIdx.x - col_ctas) * CT_ROWS;
+	const int nit = colcta ? (h + CT_CROWS - 1) / CT_CROWS : (w + CT_RCOLS - 1) / CT_RCOLS;
+	if (tid == 0) {
+		for (int st = 0; st < stages; st++) mbar_init(bar_a + 8 * st, 1);
+		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+	}
+	__syncthreads();
+	auto issue = [&](int it) {                           // thread 0 only
+		if (it >= nit) return;
+		const int slot = it % stages;
+		const unsigned bar = bar_a + 8 * slot;
+		mbar_expect_tx(bar, box_bytes);                  // out-of-bounds fill counts: always the whole box
+		if (colcta) tma_box3(ring_a + slot * box_bytes, &cmap, x0, it * CT_CROWS, f, bar);
+		else tma_box3(ring_a + slot * box_bytes, &rmap, it * CT_RCOLS, y0, f, bar);
+	};
+	if (tid == 0) for (int st = 0; st < stages - 1; st++) issue(st);
+	float acc = 0.0f;
+	const bool owner = colcta ? (tid < w - x0) : (tid < h - y0);        // one thread per column / row of the CTA
+	for (int it = 0; it < nit; it++) {
+		__syncthreads();                                 // everybody is done with the slot of stage it-1: it may be refilled
+		if (tid == 0) issue(it + stages - 1);
+		const int slot = it % stages;
+		mbar_wait(bar_a + 8 * slot, (unsigned) ((it / stages) & 1));
+		if (!owner) continue;
+		if (colcta) {
+			const float *buf = ring + slot * (CT_COLS * CT_CROWS) + tid;
+			const int rows = min(CT_CROWS, h - it * CT_CROWS);
+			if (rows == CT_CROWS) {
+				#pragma unroll
+				for (int r = 0; r < CT_CROWS; r++) acc = __fadd_rn(acc, buf[r * CT_COLS]);
+			} else for (int r = 0; r < rows; r++) acc = __fadd_rn(acc, buf[r * CT_COLS]);
+		} else {
+			// row tid is 128 B at tid * 128; its 16-byte chunk c sits at chunk position c ^ (tid & 7) (128-byte swizzle), so the
+			// eight lanes of a quarter-warp read eight different chunks: LDS.128 without bank conflicts
+			const float4 *row = reinterpret_cast<const float4 *>(ring + slot * (CT_RCOLS * CT_ROWS) + tid * CT_RCOLS);
+			const int chunks = min(CT_RCOLS, w - it * CT_RCOLS) >> 2, sw = tid & 7;
+			if (chunks == CT_RCOLS / 4) {
+				#pragma unroll
+				for (int c = 0; c < CT_RCOLS / 4; c++) {
+					const float4 q = row[c ^ sw];
+					acc = __fadd_rn(acc, q.x); acc = __fadd_rn(acc, q.y); acc = __fadd_rn(acc, q.z); acc = __fadd_rn(acc, q.w);
+				}
+			} else for (int c = 0; c < chunks; c++) {
+				const float4 q = row[c ^ sw];
+				acc = __fadd_rn(acc, q.x); acc = __fadd_rn(acc, q.y); acc = __fadd_rn(acc, q.z); acc = __fadd_rn(acc, q.w);
+			}
+		}
+	}
+	if (owner) { if (colcta) wbuf[(size_t) f * w + x0 + tid] = acc; else hbuf[(size_t) f * h + y0 + tid] = acc; }
+}
+
+// Rows at any alignment (odd widths: 1481, 507): every pixel copied with a 4-byte cp.async through a 4-stage ring.
 //   column CTA: 128 columns x all rows, stages of 16 rows, thread c owns column c;
 //   row CTA:    32 rows x all columns, stages of 64 columns (pitch 65: conflict-free), lane r of warp 0 owns row r.
-// The frame is read twice, the second time mostly from L2 (the two kinds of CTA of a frame are neighbours in the grid).
 constexpr int CL_COLS = 128, CL_CROWS = 16, CL_ROWS = 32, CL_RCOLS = 64, CL_STAGES = 4;
-constexpr int CL_RPITCH_V = CL_RCOLS + 4, CL_RPITCH_S = CL_RCOLS + 1;       // 16-byte rows read with LDS.128 / scalar rows, both conflict-free
-constexpr int CL_SMEM_FLOATS = CL_STAGES * (CL_CROWS * CL_COLS > CL_ROWS * CL_RPITCH_V ? CL_CROWS * CL_COLS : CL_ROWS * CL_RPITCH_V);
-// VEC: the frame's rows start on 16-byte boundaries (w % 4 == 0, aligned base): 16-byte cp.async and float4 reads of the
-// ring -- a quarter of the copy instructions, which is what bounds this kernel (ncu: issue slots, not DRAM).
-template <bool VEC>
+constexpr int CL_RPITCH = CL_RCOLS + 1;
+constexpr int CL_SMEM_FLOATS = CL_STAGES * (CL_CROWS * CL_COLS > CL_ROWS * CL_RPITCH ? CL_CROWS * CL_COLS : CL_ROWS * CL_RPITCH);
 __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in, int w, int h, float *__restrict__ wbuf,
                                                    float *__restrict__ hbuf, int col_ctas) {
 	__shared__ __align__(16) float ring[CL_SMEM_FLOATS];
@@ -278,16 +372,9 @@ __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in,
 				float *dst = ring + (it % CL_STAGES) * (CL_CROWS * CL_COLS);
 				const int y0 = it * CL_CROWS, rows = min(CL_CROWS, h - y0);
 				const float *s0 = src + (size_t) y0 * w + x0;
-				if (VEC) {
-					for (int idx = tid; idx < rows * (CL_COLS / 4); idx += 256) {
-						const int r = idx / (CL_COLS / 4), c = (idx % (CL_COLS / 4)) * 4;
-						if (c < cols) __pipeline_memcpy_async(dst + r * CL_COLS + c, s0 + r * w + c, 16);
-					}
-				} else {
-					for (int idx = tid; idx < rows * CL_COLS; idx += 256) {
-						const int r = idx / CL_COLS, c = idx % CL_COLS;
-						if (c < cols) __pipeline_memcpy_async(dst + idx, s0 + r * w + c, sizeof(float));
-					}
+				for (int idx = tid; idx < rows * CL_COLS; idx += 256) {
+					const int r = idx / CL_COLS, c = idx % CL_COLS;
+					if (c < cols) __pipeline_memcpy_async(dst + idx, s0 + r * w + c, sizeof(float));
 				}
 			}
 			__pipeline_commit();
@@ -310,24 +397,16 @@ __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in,
 		if (tid < cols) wbuf[(size_t) f * w + x0 + tid] = acc;
 		return;
 	}
-	constexpr int RP = VEC ? CL_RPITCH_V : CL_RPITCH_S;
 	const int y0 = ((int) blockIdx.x - col_ctas) * CL_ROWS, rows = min(CL_ROWS, h - y0);
 	const int nit = (w + CL_RCOLS - 1) / CL_RCOLS;
 	auto issue = [&](int it) {
 		if (it < nit) {
-			float *dst = ring + (it % CL_STAGES) * (CL_ROWS * RP);
+			float *dst = ring + (it % CL_STAGES) * (CL_ROWS * CL_RPITCH);
 			const int c0 = it * CL_RCOLS, cols = min(CL_RCOLS, w - c0);
 			const float *s0 = src + (size_t) y0 * w + c0;
-			if (VEC) {
-				for (int idx = tid; idx < rows * (CL_RCOLS / 4); idx += 256) {
-					const int r = idx / (CL_RCOLS / 4), c = (idx % (CL_RCOLS / 4)) * 4;
-					if (c < cols) __pipeline_memcpy_async(dst + r * RP + c, s0 + r * w + c, 16);
-				}
-			} else {
-				for (int idx = tid; idx < rows * CL_RCOLS; idx += 256) {
-					const int r = idx / CL_RCOLS, c = idx % CL_RCOLS;
-					if (c < cols) __pipeline_memcpy_async(dst + r * RP + c, s0 + r * w + c, sizeof(float));
-				}
+			for (int idx = tid; idx < rows * CL_RCOLS; idx += 256) {
+				const int r = idx / CL_RCOLS, c = idx % CL_RCOLS;
+				if (c < cols) __pipeline_memcpy_async(dst + r * CL_RPITCH + c, s0 + r * w + c, sizeof(float));
 			}
 		}
 		__pipeline_commit();
@@ -339,99 +418,15 @@ __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in,
 		__syncthreads();
 		issue(it + CL_STAGES - 1);
 		if (tid < rows) {
-			const float *buf = ring + (it % CL_STAGES) * (CL_ROWS * RP) + tid * RP;
+			const float *buf = ring + (it % CL_STAGES) * (CL_ROWS * CL_RPITCH) + tid * CL_RPITCH;
 			const int cols = min(CL_RCOLS, w - it * CL_RCOLS);
-			if (VEC) {
-				#pragma unroll 4
-				for (int c = 0; c < cols; c += 4) {
-					const float4 q = *reinterpret_cast<const float4 *>(buf + c);
-					acc = __fadd_rn(acc, q.x); acc = __fadd_rn(acc, q.y); acc = __fadd_rn(acc, q.z); acc = __fadd_rn(acc, q.w);
-				}
-			} else if (cols == CL_RCOLS) {
+			if (cols == CL_RCOLS) {
 				#pragma unroll 16
 				for (int c = 0; c < CL_RCOLS; c++) acc = __fadd_rn(acc, buf[c]);
 			} else for (int c = 0; c < cols; c++) acc = __fadd_rn(acc, buf[c]);
 		}
 	}
 	if (tid < rows) hbuf[(size_t) f * h + y0 + tid] = acc;
-}
-
-// ---- the same kernel with the copies handed to the TMA engine -----------------------------------------------------------
-// ncu on the cp.async version: bound by issue slots, i.e. by the copy instructions themselves.  Here the rows of a stage are
-// 1-D bulk copies (cp.async.bulk, SASS UBLKCP): one lane of warp 0 issues one row (512 B for a column CTA, 256 B for a row
-// CTA), completion is counted in bytes on the stage's mbarrier, the owner threads wait on it and add.  128 threads per CTA:
-// nobody is needed for copying.  Requires 16-byte aligned rows (w % 4 == 0), as the VEC variant.  Measured slower than the
-// cp.async ring at this slab shape (many small rows: the TMA unit's request rate binds), hence opt-in (TSDRGPU_COLLAPSE_TMA=1).
-__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
-	asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
-	             :: "r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_row(unsigned dst_smem, const void *src, unsigned bytes, unsigned bar) {
-	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-	             :: "r"(dst_smem), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-constexpr int CL_TMA_THREADS = 128;
-__global__ void __launch_bounds__(CL_TMA_THREADS) fs_collapse_tma(const float *__restrict__ in, int w, int h, float *__restrict__ wbuf,
-                                                                  float *__restrict__ hbuf, int col_ctas) {
-	__shared__ __align__(128) float ring[CL_SMEM_FLOATS];
-	__shared__ __align__(8) unsigned long long bars[CL_STAGES];
-	const int f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-	const float *src = in + (size_t) f * w * h;
-	const unsigned ring_a = (unsigned) __cvta_generic_to_shared(ring), bar_a = (unsigned) __cvta_generic_to_shared(bars);
-	if (tid == 0) {
-		for (int st = 0; st < CL_STAGES; st++) mbar_init(bar_a + 8 * st, 1);
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
-	__syncthreads();
-	const bool colcta = (int) blockIdx.x < col_ctas;
-	// geometry of this CTA's slab: `nrows` rows per stage of `rowbytes` bytes, `nit` stages
-	const int x0 = colcta ? blockIdx.x * CL_COLS : 0, y0 = colcta ? 0 : ((int) blockIdx.x - col_ctas) * CL_ROWS;
-	const int cols = colcta ? min(CL_COLS, w - x0) : 0, rows = colcta ? 0 : min(CL_ROWS, h - y0);
-	const int nit = colcta ? (h + CL_CROWS - 1) / CL_CROWS : (w + CL_RCOLS - 1) / CL_RCOLS;
-	auto issue = [&](int it) {                           // warp 0 only
-		if (it >= nit) return;
-		const unsigned bar = bar_a + 8 * (it % CL_STAGES);
-		if (colcta) {
-			const int r0 = it * CL_CROWS, nr = min(CL_CROWS, h - r0);
-			if (lane == 0) mbar_expect_tx(bar, (unsigned) (nr * cols * 4));
-			__syncwarp();
-			if (lane < nr) tma_row(ring_a + 4u * (unsigned) ((it % CL_STAGES) * (CL_CROWS * CL_COLS) + lane * CL_COLS), src + (size_t) (r0 + lane) * w + x0, (unsigned) (cols * 4), bar);
-		} else {
-			const int c0 = it * CL_RCOLS, nc = min(CL_RCOLS, w - c0);
-			if (lane == 0) mbar_expect_tx(bar, (unsigned) (rows * nc * 4));
-			__syncwarp();
-			if (lane < rows) tma_row(ring_a + 4u * (unsigned) ((it % CL_STAGES) * (CL_ROWS * CL_RPITCH_V) + lane * CL_RPITCH_V), src + (size_t) (y0 + lane) * w + c0, (unsigned) (nc * 4), bar);
-		}
-	};
-	if (warp == 0) for (int st = 0; st < CL_STAGES - 1; st++) issue(st);
-	float acc = 0.0f;
-	const bool owner = colcta ? (tid < cols) : (tid < rows);
-	for (int it = 0; it < nit; it++) {
-		__syncthreads();                                 // everybody is done with the buffer of stage it-1: it may be refilled
-		if (warp == 0) issue(it + CL_STAGES - 1);
-		if (owner) {
-			mbar_wait(bar_a + 8 * (it % CL_STAGES), (unsigned) ((it / CL_STAGES) & 1));
-			if (colcta) {
-				const float *buf = ring + (it % CL_STAGES) * (CL_CROWS * CL_COLS) + tid;
-				const int nr = min(CL_CROWS, h - it * CL_CROWS);
-				if (nr == CL_CROWS) {
-					#pragma unroll
-					for (int r = 0; r < CL_CROWS; r++) acc = __fadd_rn(acc, buf[r * CL_COLS]);
-				} else for (int r = 0; r < nr; r++) acc = __fadd_rn(acc, buf[r * CL_COLS]);
-			} else {
-				const float *buf = ring + (it % CL_STAGES) * (CL_ROWS * CL_RPITCH_V) + tid * CL_RPITCH_V;
-				const int nc = min(CL_RCOLS, w - it * CL_RCOLS);
-				#pragma unroll 4
-				for (int c = 0; c < nc; c += 4) {
-					const float4 q = *reinterpret_cast<const float4 *>(buf + c);
-					acc = __fadd_rn(acc, q.x); acc = __fadd_rn(acc, q.y); acc = __fadd_rn(acc, q.z); acc = __fadd_rn(acc, q.w);
-				}
-			}
-		}
-	}
-	if (owner) { if (colcta) wbuf[(size_t) f * w + x0 + tid] = acc; else hbuf[(size_t) f * h + y0 + tid] = acc; }
 }
 
 // ---------------------------------------------------------------- sync search (syncdetector.c:26-153, gaussian.c)
@@ -971,9 +966,49 @@ __global__ void fs_results_autogain(int nframes, const FrameParams *__restrict__
 }
 
 // ---------------------------------------------------------------- circular 2-D re-centre (syncdetector.c:187-207)
+// 16-byte rows (w % 4 == 0, aligned in / out): a CTA copies a band of `band` destination rows of one frame, viewed as one run of
+// band * w/4 float4s, four of them in flight per thread.  Destination float4 j of a row takes pixels (4j + dx .. 4j + dx + 3) mod w of
+// its source row: with a = dx & 3 these are the last 4 - a of aligned source float4 s and the first a of the next one (the
+// row's first float4 after the last), so every load and store is 16 bytes and the second load of a lane is mostly its
+// neighbour's first, from L1.
+__global__ void __launch_bounds__(256) fs_shift4(const float *__restrict__ in, float *__restrict__ out, int w, int h, int band,
+                                                 const tsdrgpu_frame_result_t *__restrict__ results) {
+	const int f = blockIdx.y;
+	const int dx = results[f].x_dx, dy = results[f].y_dx;
+	const int w4 = w >> 2, a = dx & 3, s0 = dx >> 2;
+	const int y0 = blockIdx.x * band, rows = min(band, h - y0);
+	const size_t n = (size_t) w * h;
+	const float4 *src = reinterpret_cast<const float4 *>(in + f * n);
+	float4 *dst = reinterpret_cast<float4 *>(out + f * n + (size_t) y0 * w);
+	const int items = rows * w4;
+	for (int i0 = threadIdx.x; i0 < items; i0 += 4 * 256) {
+		float4 v[4];
+		#pragma unroll
+		for (int u = 0; u < 4; u++) {
+			const int i = i0 + u * 256;
+			if (i < items) {
+				const int r = i / w4, j = i - r * w4;
+				int sy = y0 + r + dy; if (sy >= h) sy -= h;
+				const float4 *srow = src + (size_t) sy * w4;
+				int s = j + s0; if (s >= w4) s -= w4;
+				const float4 lo = __ldg(srow + s);
+				if (a == 0) v[u] = lo;
+				else {
+					const float4 hi = __ldg(srow + (s + 1 == w4 ? 0 : s + 1));
+					v[u] = (a == 1) ? make_float4(lo.y, lo.z, lo.w, hi.x) : (a == 2) ? make_float4(lo.z, lo.w, hi.x, hi.y)
+					                                                                 : make_float4(lo.w, hi.x, hi.y, hi.z);
+				}
+			}
+		}
+		#pragma unroll
+		for (int u = 0; u < 4; u++) if (i0 + u * 256 < items) dst[i0 + u * 256] = v[u];
+	}
+}
+
+// rows at any alignment (odd widths): one destination row per CTA iteration
 __global__ void __launch_bounds__(256) fs_shift(const float *__restrict__ in, float *__restrict__ out, int w, int h,
                                                 const tsdrgpu_frame_result_t *__restrict__ results) {
-	// one destination row per CTA iteration: no division per pixel, the wrap is a compare; up to 4 loads in flight per thread
+	// no division per pixel, the wrap is a compare; up to 4 loads in flight per thread
 	const int f = blockIdx.y;
 	const int dx = results[f].x_dx, dy = results[f].y_dx;
 	const size_t n = (size_t) w * h;
@@ -1074,6 +1109,63 @@ inline unsigned grid_for(size_t n, int sm_count, int per_sm = 8) {
 	return (unsigned) (want < cap ? (want ? want : 1) : cap);
 }
 
+// fs_collapse_tiles' two tensor maps over a batch of frames (w % 4 == 0 and a 16-byte aligned base: row and frame strides are
+// multiples of 16 bytes, as the TMA unit requires).  cuTensorMapEncodeTiled comes from the driver through the runtime's
+// entry-point query, so the library does not link libcuda.
+struct CollapseMaps {
+	const void *ptr; int w, h, nframes;
+	CUtensorMap col, row;
+};
+
+int encode_collapse_maps(tsdrgpu_ctx_t *ctx, const float *ptr, int w, int h, int nframes, CollapseMaps *m) {
+	static PFN_cuTensorMapEncodeTiled_v12000 encode = NULL;
+	if (!encode) {
+		void *fn = NULL;
+		cudaDriverEntryPointQueryResult q;
+		CU_TRY(ctx, cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q));
+		if (q != cudaDriverEntryPointSuccess || !fn)
+			return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "cuTensorMapEncodeTiled not found in the driver", cudaSuccess, __FILE__, __LINE__);
+		encode = (PFN_cuTensorMapEncodeTiled_v12000) fn;
+	}
+	const cuuint64_t dims[3] = {(cuuint64_t) w, (cuuint64_t) h, (cuuint64_t) nframes};
+	const cuuint64_t strides[2] = {(cuuint64_t) w * 4, (cuuint64_t) w * h * 4};
+	const cuuint32_t cbox[3] = {CT_COLS, CT_CROWS, 1}, rbox[3] = {CT_RCOLS, CT_ROWS, 1}, unit[3] = {1, 1, 1};
+	CUresult r = encode(&m->col, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *) ptr, dims, strides, cbox, unit, CU_TENSOR_MAP_INTERLEAVE_NONE,
+	                    CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+	if (r == CUDA_SUCCESS)
+		r = encode(&m->row, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *) ptr, dims, strides, rbox, unit, CU_TENSOR_MAP_INTERLEAVE_NONE,
+		           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+	if (r != CUDA_SUCCESS) return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "cuTensorMapEncodeTiled (collapse)", cudaSuccess, __FILE__, __LINE__);
+	m->ptr = ptr; m->w = w; m->h = h; m->nframes = nframes;
+	return TSDRGPU_OK;
+}
+
+// row and column sums of `nframes` frames: the tensor-map kernel on 16-byte rows, the cp.async kernel otherwise
+int launch_collapse(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *src, int w, int h, int nframes, float *wbuf, float *hbuf,
+                    CollapseMaps *cache, int ncache) {
+	if ((w % 4 == 0) && ((reinterpret_cast<unsigned long long>(src) & 15ull) == 0)) {
+		CollapseMaps local, *m = NULL;
+		for (int i = 0; i < ncache && !m; i++)
+			if (cache[i].ptr == src && cache[i].w == w && cache[i].h == h && cache[i].nframes == nframes) m = &cache[i];
+		if (!m) {
+			m = &local;
+			if (ncache) {                                // the frame stage collapses a handful of buffers: evict the oldest
+				for (int i = ncache - 1; i > 0; i--) cache[i] = cache[i - 1];
+				m = &cache[0];
+			}
+			int rc = encode_collapse_maps(ctx, src, w, h, nframes, m);
+			if (rc) { m->ptr = NULL; return rc; }
+		}
+		const int col_ctas = (w + CT_COLS - 1) / CT_COLS, row_ctas = (h + CT_ROWS - 1) / CT_ROWS;
+		CU_TRY(ctx, cudaFuncSetAttribute(fs_collapse_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
+		KL(ctx, "fs_collapse", stream, fs_collapse_tiles<<<dim3(col_ctas + row_ctas, nframes), CT_THREADS, CT_SMEM, stream>>>(m->col, m->row, w, h, wbuf, hbuf, col_ctas));
+	} else {
+		const int col_ctas = (w + CL_COLS - 1) / CL_COLS, row_ctas = (h + CL_ROWS - 1) / CL_ROWS;
+		KL(ctx, "fs_collapse", stream, fs_collapse<<<dim3(col_ctas + row_ctas, nframes), 256, 0, stream>>>(src, w, h, wbuf, hbuf, col_ctas));
+	}
+	return TSDRGPU_OK;
+}
+
 }  // namespace
 
 // -----------------------------------------------------------------------------------------------------------------
@@ -1098,6 +1190,7 @@ struct tsdrgpu_framestage {
 	cudaStream_t s_side;
 	cudaEvent_t ev_ready[2];                     // main: collapse of this phase done -> side may start
 	cudaEvent_t ev_done[2];                      // side: sync + emit of this phase done -> buffers of the phase are free
+	CollapseMaps collapse_maps[4];               // fs_collapse_tiles' tensor maps of the buffers collapsed last (d_t2[0/1], d_t1)
 };
 
 static int fs_reserve(tsdrgpu_framestage *fs, int nframes, size_t n, int w, int h) {
@@ -1277,7 +1370,6 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 	tsdrgpu_frame_result_t *d_results = fs->d_results[ph];
 	const double fresh = 1.0 - (double) motionblur;      // dsp.c:29
 	const int minsize_x = (int) (w * 0.05f), minsize_y = (int) (h * 0.01f);   // syncdetector.c:178-179
-	const int col_ctas = (w + CL_COLS - 1) / CL_COLS, row_ctas = (h + CL_ROWS - 1) / CL_ROWS;
 	const size_t prep_smem = sizeof(double) * ((size_t) w + h + 2);
 	const size_t rec_bytes = sizeof(double) * fs_prep_stride(w, h);
 	const int sync_nbuf = (2 * rec_bytes <= 96 * 1024) ? 2 : 1;     // prefetch one frame ahead while two records fit beside the main stream's CTAs
@@ -1290,13 +1382,7 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 
 	// collapse on `stream`, then sync search on `s2` (== stream unless overlapped)
 	auto collapse_sync = [&](const float *src, cudaStream_t s2) -> int {
-		const bool cvec = (w % 4 == 0) && ((reinterpret_cast<unsigned long long>(src) & 15ull) == 0);
-		// 64 frames of 740x1125 are 1.3 M bulk copies of 256-512 B per launch, bound by the TMA unit's request rate: the cp.async
-		// variant is the default and TMA is opt-in
-		const bool use_tma = getenv("TSDRGPU_COLLAPSE_TMA") != NULL;
-		if (cvec && use_tma) KL(ctx, "fs_collapse", stream, fs_collapse_tma<<<dim3(col_ctas + row_ctas, nframes), CL_TMA_THREADS, 0, stream>>>(src, w, h, fs->d_wstrips[ph], fs->d_hstrips[ph], col_ctas));
-		else if (cvec) KL(ctx, "fs_collapse", stream, fs_collapse<true><<<dim3(col_ctas + row_ctas, nframes), 256, 0, stream>>>(src, w, h, fs->d_wstrips[ph], fs->d_hstrips[ph], col_ctas));
-		else KL(ctx, "fs_collapse", stream, fs_collapse<false><<<dim3(col_ctas + row_ctas, nframes), 256, 0, stream>>>(src, w, h, fs->d_wstrips[ph], fs->d_hstrips[ph], col_ctas));
+		if ((rc = launch_collapse(ctx, stream, src, w, h, nframes, fs->d_wstrips[ph], fs->d_hstrips[ph], fs->collapse_maps, 4))) return rc;
 		if (s2 != stream) {
 			CU_TRY(ctx, cudaEventRecord(fs->ev_ready[ph], stream));
 			CU_TRY(ctx, cudaStreamWaitEvent(s2, fs->ev_ready[ph], 0));
@@ -1312,7 +1398,12 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 	// syncdetector_run's output stage: src -> dst (dst != src), or in place on src when allowed
 	auto emit = [&](float *src, float *dst, bool greenlines, bool may_modify, float **result, cudaStream_t s2) -> int {
 		if (autoshift) {
-			KL(ctx, "fs_shift", s2, fs_shift<<<dim3((unsigned) h, nframes), 256, 0, s2>>>(src, dst, w, h, d_results));
+			if ((w % 4 == 0) && (((reinterpret_cast<unsigned long long>(src) | reinterpret_cast<unsigned long long>(dst)) & 15ull) == 0)) {
+				// bands of rows, about one wave of 8 CTAs per SM over the batch
+				const int want = (int) ((ctx->sm_count * 8 + nframes - 1) / nframes);
+				const int band = (h + (want < h ? want : h) - 1) / (want < h ? want : h), bands = (h + band - 1) / band;
+				KL(ctx, "fs_shift", s2, fs_shift4<<<dim3((unsigned) bands, nframes), 256, 0, s2>>>(src, dst, w, h, band, d_results));
+			} else KL(ctx, "fs_shift", s2, fs_shift<<<dim3((unsigned) h, nframes), 256, 0, s2>>>(src, dst, w, h, d_results));
 			*result = dst;
 		} else if (greenlines && may_modify) {
 			KL(ctx, "fs_greenlines", s2, fs_greenlines<<<dim3(8, nframes), 256, 0, s2>>>(src, w, h, d_results));
@@ -1432,11 +1523,7 @@ int tsdrgpu_timelowpass(tsdrgpu_ctx_t *ctx, void *stream, float coeff, int n, co
 int tsdrgpu_average_v_h(tsdrgpu_ctx_t *ctx, void *stream, int w, int h, const float *d_in, float *d_wbuf, float *d_hbuf) {
 	BIND(ctx);
 	ARG_TRY(ctx, w > 0 && h > 0 && d_in && d_wbuf && d_hbuf);
-	const int col_ctas = (w + CL_COLS - 1) / CL_COLS, row_ctas = (h + CL_ROWS - 1) / CL_ROWS;
-	if ((w % 4 == 0) && ((reinterpret_cast<unsigned long long>(d_in) & 15ull) == 0))
-		KL(ctx, "fs_collapse", (cudaStream_t) stream, fs_collapse<true><<<dim3(col_ctas + row_ctas, 1), 256, 0, (cudaStream_t) stream>>>(d_in, w, h, d_wbuf, d_hbuf, col_ctas));
-	else KL(ctx, "fs_collapse", (cudaStream_t) stream, fs_collapse<false><<<dim3(col_ctas + row_ctas, 1), 256, 0, (cudaStream_t) stream>>>(d_in, w, h, d_wbuf, d_hbuf, col_ctas));
-	return TSDRGPU_OK;
+	return launch_collapse(ctx, (cudaStream_t) stream, d_in, w, h, 1, d_wbuf, d_hbuf, NULL, 0);
 }
 
 int tsdrgpu_gaussianblur(tsdrgpu_ctx_t *ctx, void *stream, float *d_data, int n) {
