@@ -5,9 +5,7 @@ There is no fallback of any kind: a missing library or a missing CUDA device rai
 from __future__ import annotations
 
 import ctypes as C
-import math
 import os
-import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libtsdrgpu.so")
@@ -48,22 +46,11 @@ RESAMPLER_KERNELS = {"box": 0, "sinc": 1}          # TSDRGPU_RS_BOX / TSDRGPU_RS
 AG_MINMAX, AG_CLIP, AG_MAX_PPM = 0, 1, 250000      # TSDRGPU_AG_MINMAX / TSDRGPU_AG_CLIP / TSDRGPU_AG_MAX_PPM
 
 
-_PERCENT = re.compile(r"[0-9]+(\.[0-9]+)?")
-
-
-def autogain_ppm(percent: str) -> int:
-    """tsdrgpu_autogain_ppm restated: digits with an optional fraction, value in [0, 25] -> floor(percent * 1e4 + 0.5); else -1."""
-    if not _PERCENT.fullmatch(percent):
-        return -1
-    v = float(percent)
-    return math.floor(v * 1e4 + 0.5) if v <= 25.0 else -1
-
-
 def autogain_mode(spec: str):
-    """"minmax" or "clip:<percent>" (the host library's TSDR_AUTOGAIN spelling) -> (mode, ppm)."""
+    """"minmax" or "clip:<percent>" (the host library's TSDR_AUTOGAIN spelling) -> (mode, ppm), read by tsdrgpu_autogain_ppm."""
     if spec == "minmax":
         return AG_MINMAX, 0
-    ppm = autogain_ppm(spec[5:]) if spec.startswith("clip:") else -1
+    ppm = lib().tsdrgpu_autogain_ppm(spec[5:].encode()) if spec.startswith("clip:") else -1
     if ppm < 0:
         raise ValueError(f"auto-gain must be 'minmax' or 'clip:<percent>' with percent in [0, 25], not {spec!r}")
     return AG_CLIP, ppm

@@ -84,10 +84,37 @@ __device__ __forceinline__ float ldg_stream_f1(const float *p) {
 	return v;
 }
 
-// ---- internal entry points shared between translation units (fft.cu owns the transforms)
+// ---- pixels of the frame stage
+__device__ __forceinline__ bool px_is_marker(float v) { return v > 250.0f || v < -250.0f; }   // dsp.c:57
+// the pixels the clip auto-gain, CLAHE and NLM work on (tsdrgpu.h): neither a marker nor NaN
+__device__ __forceinline__ bool px_valid(float v) { return !px_is_marker(v) && v == v; }
+
+// n floats from src cut on the ADDRESS into a scalar head up to the next 16-byte boundary, a float4 body and a scalar tail
+// from tail0: frames of an odd number of pixels start at any of the four 4-byte phases
+struct F4Split {
+	size_t head, nbody, tail0, n;
+	__device__ F4Split(const float *src, size_t count) : n(count) {
+		head = (size_t) ((4u - (unsigned) ((reinterpret_cast<unsigned long long>(src) >> 2) & 3ull)) & 3u);
+		if (head > n) head = n;
+		nbody = (n - head) >> 2; tail0 = head + (nbody << 2);
+	}
+};
+
+// ---- internal entry points shared between translation units (fft.cu owns the transforms, framestage.cu fs_copy)
 constexpr unsigned TSDRGPU_ARGMAX_PARTS = 1024;
 int tsdrgpu_fft_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, unsigned long long n_pow2, int inverse);
 int tsdrgpu_fft_oop_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, unsigned long long n_pow2, int inverse);
 int tsdrgpu_fft_batch_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, long long in_bs, float2 *out, long long out_bs,
                                float2 *scratch, unsigned long long n_pow2, unsigned batch, int inverse);
 int tsdrgpu_argmax_mag_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *x, unsigned n, void *d_part, int *d_result);
+int fs_copy_async(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, size_t total);
+// enhance.cu: NLM then CLAHE on delivered frames, modes and parameters as the frame stage's setters take them
+struct EnhanceState {
+	int contrast, clip_centi, tx, ty;            // TSDRGPU_CONTRAST_* and its parameters
+	int denoise, h_milli, r, p;                  // TSDRGPU_DENOISE_* and its parameters (R, P)
+	unsigned *d_clahe; size_t clahe_bytes;       // CLAHE histograms / LUTs of one pass
+	float *d_nlm; size_t nlm_bytes;              // NLM output of a batch
+};
+int enhance_reserve(tsdrgpu_ctx_t *ctx, EnhanceState *st, int nframes, int w, int h);
+int enhance_run(tsdrgpu_ctx_t *ctx, const EnhanceState *st, cudaStream_t stream, float *d_frames, int nframes, int w, int h);
+void enhance_free(EnhanceState *st);

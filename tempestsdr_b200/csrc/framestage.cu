@@ -21,7 +21,6 @@
 // memory (tensor-map or cp.async copies) for the order-bound row/column sums, grid sized by pixels x frames.
 #include "common.cuh"
 #include "host_plan.h"
-#include <math.h>
 #include <stdlib.h>
 #include <cuda_pipeline.h>
 #include <cuda.h>
@@ -34,8 +33,6 @@ namespace {
 constexpr int FS_MAX_STRIP = 8192;      // longest width/height the in-CTA sync search supports
 constexpr int FS_MM_CHUNKS = 64;        // partial reductions per frame
 constexpr int FS_SYNC_THREADS = 512;       // half an SM's registers: it must find room beside the main stream's CTAs
-
-__device__ __forceinline__ bool px_is_marker(float v) { return v > 250.0f || v < -250.0f; }   // dsp.c:57
 
 struct SyncState {                      // device-resident syncdetector_t + dsp_autogain_t
 	int x_dx, x_vx, x_absvx, x_strip;
@@ -69,13 +66,11 @@ __global__ void __launch_bounds__(256) fs_minmax(const float *__restrict__ in, s
 	};
 	{
 		const size_t gtid = (size_t) blockIdx.x * blockDim.x + threadIdx.x, gsz = (size_t) gridDim.x * blockDim.x;
-		size_t head = (size_t) ((4u - (unsigned) ((reinterpret_cast<unsigned long long>(src) >> 2) & 3ull)) & 3u);
-		if (head > n) head = n;
-		const size_t nbody = (n - head) >> 2, tail0 = head + (nbody << 2);
-		if (gtid < head) take(__ldg(src + gtid));
-		if (gtid < n - tail0) take(__ldg(src + tail0 + gtid));
-		const float4 *src4 = reinterpret_cast<const float4 *>(src + head);
-		for (size_t i = gtid; i < nbody; i += gsz) {
+		const F4Split s(src, n);
+		if (gtid < s.head) take(__ldg(src + gtid));
+		if (gtid < n - s.tail0) take(__ldg(src + s.tail0 + gtid));
+		const float4 *src4 = reinterpret_cast<const float4 *>(src + s.head);
+		for (size_t i = gtid; i < s.nbody; i += gsz) {
 			const float4 q = __ldg(src4 + i);
 			take(q.x); take(q.y); take(q.z); take(q.w);
 		}
@@ -234,7 +229,7 @@ __global__ void __launch_bounds__(256) fs_select_hist(const float *__restrict__ 
 		const bool marker = px_is_marker(v);
 		if (SNR && inside && !marker) sum += (double) v;   // the SNR's mean keeps the reference's terms (NaN included, dsp.c:58-60)
 		unsigned bin = ~0u;
-		if (inside && !marker && v == v) {
+		if (inside && !marker && v == v) {            // px_valid(v), reusing the marker test above
 			const unsigned k = sel_key(v);
 			if (R == 1) bin = k >> 21;
 			else {
@@ -249,15 +244,13 @@ __global__ void __launch_bounds__(256) fs_select_hist(const float *__restrict__ 
 	{   // 16-byte loads on the address, scalar head and tail (as fs_minmax); loop trip counts are warp-uniform
 		const size_t gtid = (size_t) blockIdx.x * blockDim.x + threadIdx.x, gsz = (size_t) gridDim.x * blockDim.x;
 		const size_t lane = threadIdx.x & 31;
-		size_t head = (size_t) ((4u - (unsigned) ((reinterpret_cast<unsigned long long>(src) >> 2) & 3ull)) & 3u);
-		if (head > n) head = n;
-		const size_t nbody = (n - head) >> 2, tail0 = head + (nbody << 2);
-		take(gtid < head ? __ldg(src + gtid) : 0.0f, gtid < head);
-		take(gtid < n - tail0 ? __ldg(src + tail0 + gtid) : 0.0f, gtid < n - tail0);
-		const float4 *src4 = reinterpret_cast<const float4 *>(src + head);
-		for (size_t i0 = gtid - lane; i0 < nbody; i0 += gsz) {
+		const F4Split s(src, n);
+		take(gtid < s.head ? __ldg(src + gtid) : 0.0f, gtid < s.head);
+		take(gtid < n - s.tail0 ? __ldg(src + s.tail0 + gtid) : 0.0f, gtid < n - s.tail0);
+		const float4 *src4 = reinterpret_cast<const float4 *>(src + s.head);
+		for (size_t i0 = gtid - lane; i0 < s.nbody; i0 += gsz) {
 			const size_t i = i0 + lane;
-			const bool inside = i < nbody;
+			const bool inside = i < s.nbody;
 			const float4 q = inside ? __ldg(src4 + i) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 			take(q.x, inside); take(q.y, inside); take(q.z, inside); take(q.w, inside);
 		}
@@ -1337,322 +1330,12 @@ int launch_collapse(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *src, i
 	return TSDRGPU_OK;
 }
 
-// ---------------------------------------------------------------- CLAHE (beyond the reference; the definition is in tsdrgpu.h)
-// Per pass of nf frames the histogram buffer holds [frame][tile row][tile column][256] counts, zeroed before fs_clahe_hist;
-// fs_clahe_lut overwrites each tile's counts with its LUT (floats) in place, and fs_clahe_map reads the LUTs.
-constexpr int CH_BINS = 256;
-constexpr int CH_STAGE_BYTES = 96 * 1024;        // fs_clahe_map stages up to three tile rows of LUTs when they fit in this
-constexpr size_t CH_PASS_WORDS = (size_t) 1 << 24;   // histogram words per pass (64 MB): frames are processed in passes
-
-__device__ __forceinline__ bool ch_valid(float v) { return !(v > 250.0f || v < -250.0f) && v == v; }
-__device__ __forceinline__ int ch_bin(float v) { return v <= 0.0f ? 0 : (v >= 1.0f ? CH_BINS - 1 : (int) __fmul_rn(v, 256.0f)); }
-// tile bound x_j = floor(j W / T); the tile holding pixel x is the last j with x_j <= x
-__device__ __forceinline__ int ch_bound(int j, int W, int T) { return (int) (((long long) j * W) / T); }
-__device__ __forceinline__ int ch_tile_of(int x, int W, int T) { return (int) (((long long) (x + 1) * T - 1) / W); }
-
-// interpolation along one axis for pixel x: the two tiles whose centres bracket it and the weight of the second.
-// s_j = x_j + x_{j+1} and c = 2x + 1 are twice the centres, so everything is an integer until the one division.
-__device__ __forceinline__ void ch_axis(int x, int W, int T, unsigned char *j0, unsigned char *j1, float *wt) {
-	const int c = 2 * x + 1;
-	const int s_first = ch_bound(0, W, T) + ch_bound(1, W, T), s_last = ch_bound(T - 1, W, T) + ch_bound(T, W, T);
-	if (c <= s_first) { *j0 = *j1 = 0; *wt = 0.0f; return; }
-	if (c >= s_last) { *j0 = *j1 = (unsigned char) (T - 1); *wt = 0.0f; return; }
-	const int t = ch_tile_of(x, W, T);
-	const int j = (ch_bound(t, W, T) + ch_bound(t + 1, W, T) <= c) ? t : t - 1;     // s_{t+1} > c and s_{t-1} < c always
-	const int a = ch_bound(j, W, T) + ch_bound(j + 1, W, T), b = ch_bound(j + 1, W, T) + ch_bound(j + 2, W, T);
-	*j0 = (unsigned char) j; *j1 = (unsigned char) (j + 1);
-	*wt = __fdiv_rn((float) (c - a), (float) (b - a));
-}
-
-// a CTA's pixel range: rows [r0, r1) of frame blockIdx.y, cut into an address-aligned scalar head, float4 body and scalar tail
-struct ChBand {
-	size_t head, nbody, tail0, n;
-	__device__ ChBand(const float *src, size_t count) : n(count) {
-		head = (size_t) ((4u - (unsigned) ((reinterpret_cast<unsigned long long>(src) >> 2) & 3ull)) & 3u);
-		if (head > n) head = n;
-		nbody = (n - head) >> 2; tail0 = head + (nbody << 2);
-	}
-};
-
-// histograms: grid (TY * parts, frames).  CTA (i * parts + p, f) counts part p of tile row i of frame f into TX shared
-// histograms, and adds its non-zero counts to the pass buffer once at the end.  Dynamic shared memory: TX * 1 KB + W bytes.
-__global__ void __launch_bounds__(256) fs_clahe_hist(const float *__restrict__ in, int W, int H, int TX, int TY, int parts,
-                                                     unsigned *__restrict__ hist) {
-	extern __shared__ __align__(16) unsigned ch_smem[];
-	unsigned *s_h = ch_smem;
-	unsigned char *s_col = reinterpret_cast<unsigned char *>(s_h + TX * CH_BINS);
-	const int f = blockIdx.y, i = blockIdx.x / parts, p = blockIdx.x % parts;
-	const int y0 = ch_bound(i, H, TY), rows = ch_bound(i + 1, H, TY) - y0;
-	const int r0 = y0 + (int) ((long long) p * rows / parts), r1 = y0 + (int) ((long long) (p + 1) * rows / parts);
-	for (int k = threadIdx.x; k < TX * CH_BINS; k += blockDim.x) s_h[k] = 0;
-	for (int x = threadIdx.x; x < W; x += blockDim.x) s_col[x] = (unsigned char) ch_tile_of(x, W, TX);
-	__syncthreads();
-	const float *src = in + (size_t) f * W * H + (size_t) r0 * W;
-	const ChBand band(src, (size_t) (r1 - r0) * W);
-	const unsigned uw = (unsigned) W;
-	const int lane = threadIdx.x & 31;
-	if (threadIdx.x < band.head) { const float v = src[threadIdx.x]; if (ch_valid(v)) atomicAdd(&s_h[s_col[threadIdx.x % uw] * CH_BINS + ch_bin(v)], 1u); }
-	if (threadIdx.x < band.n - band.tail0) {
-		const unsigned q = (unsigned) (band.tail0 + threadIdx.x);
-		const float v = src[q];
-		if (ch_valid(v)) atomicAdd(&s_h[s_col[q % uw] * CH_BINS + ch_bin(v)], 1u);
-	}
-	auto key_of = [&](float v, int x) { return ch_valid(v) ? s_col[x] * CH_BINS + ch_bin(v) : -1; };
-	const float4 *src4 = reinterpret_cast<const float4 *>(src + band.head);
-	for (size_t base = threadIdx.x & ~31u; base < band.nbody; base += blockDim.x) {      // warp-uniform trip count
-		const size_t k = base + lane;
-		int key[4] = {-1, -1, -1, -1};
-		if (k < band.nbody) {
-			const float4 v = __ldg(src4 + k);
-			int x = (int) ((unsigned) (band.head + 4 * k) % uw);
-			key[0] = key_of(v.x, x); x = (x + 1 == W) ? 0 : x + 1;
-			key[1] = key_of(v.y, x); x = (x + 1 == W) ? 0 : x + 1;
-			key[2] = key_of(v.z, x); x = (x + 1 == W) ? 0 : x + 1;
-			key[3] = key_of(v.w, x);
-		}
-		// a warp whose valid pixels all share one (tile, bin), as in blanking and flat areas, adds them with one atomic;
-		// otherwise each lane adds one atomic per run of equal keys among its four pixels
-		const int k0 = __shfl_sync(0xffffffffu, key[0], 0);
-		unsigned mine = 0;
-		bool only = true;
-#pragma unroll
-		for (int p = 0; p < 4; p++) { if (key[p] == k0) mine++; else if (key[p] >= 0) only = false; }
-		if (__all_sync(0xffffffffu, only) && k0 >= 0) {
-			const unsigned total = __reduce_add_sync(0xffffffffu, mine);
-			if (lane == 0) atomicAdd(&s_h[k0], total);
-		} else {
-			int run = key[0];
-			unsigned cnt = 1;
-#pragma unroll
-			for (int p = 1; p < 4; p++) {
-				if (key[p] == run) cnt++;
-				else { if (run >= 0) atomicAdd(&s_h[run], cnt); run = key[p]; cnt = 1; }
-			}
-			if (run >= 0) atomicAdd(&s_h[run], cnt);
-		}
-	}
-	__syncthreads();
-	unsigned *g = hist + ((size_t) f * TY + i) * TX * CH_BINS;
-	for (int k = threadIdx.x; k < TX * CH_BINS; k += blockDim.x) if (s_h[k]) atomicAdd(g + k, s_h[k]);
-}
-
-__device__ __forceinline__ unsigned ch_block_sum(unsigned v, unsigned *s_w) {
-	for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-	__syncthreads();                                     // s_w is free again
-	if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
-	__syncthreads();
-	unsigned t = 0;
-	for (int k = 0; k < CH_BINS / 32; k++) t += s_w[k];
-	return t;
-}
-
-// LUTs: one 256-thread CTA per (tile, frame), thread b owns bin b.  Clip at L, spread the excess in OpenCV's integer scheme
-// (closed form of its residual loop), inclusive scan, one IEEE division per bin.  The LUT overwrites the counts.
-__global__ void __launch_bounds__(CH_BINS) fs_clahe_lut(unsigned *hist, int clip_centi) {
-	__shared__ unsigned s_w[CH_BINS / 32];
-	unsigned *h = hist + ((size_t) blockIdx.y * gridDim.x + blockIdx.x) * CH_BINS;
-	const unsigned b = threadIdx.x;
-	unsigned c = h[b];
-	const unsigned nt = ch_block_sum(c, s_w);
-	float lut;
-	if (nt == 0) lut = __fdiv_rn((float) b, 255.0f);
-	else {                                               // block-uniform branch
-		const unsigned long long l = (unsigned long long) clip_centi * nt / 25600ull;
-		const unsigned L = l > 1ull ? (unsigned) l : 1u;
-		const unsigned excess = ch_block_sum(c > L ? c - L : 0u, s_w);
-		c = (c < L ? c : L) + excess / CH_BINS;
-		const unsigned r = excess % CH_BINS;
-		if (r) { const unsigned step = (CH_BINS / r > 1u) ? CH_BINS / r : 1u; if (b % step == 0 && b / step < r) c++; }
-		unsigned s = c;
-		const int lane = b & 31, wid = b >> 5;
-		for (int o = 1; o < 32; o <<= 1) { const unsigned t = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += t; }
-		__syncthreads();
-		if (lane == 31) s_w[wid] = s;
-		__syncthreads();
-		for (int k = 0; k < wid; k++) s += s_w[k];
-		lut = __fdiv_rn((float) s, (float) nt);
-	}
-	h[b] = __float_as_uint(lut);
-}
-
-// mapping: grid (bands, frames), band rows [b * bh, min(H, (b + 1) * bh)).  Per-column and per-row (tile pair, weight) tables
-// in shared memory; the LUTs of the tile rows the band touches are staged in shared memory when there are at most stage_rows
-// of them, otherwise gathered from global memory (L1).  VEC: in and out share their 16-byte phase, so the body is float4s.
-template <bool VEC>
-__global__ void __launch_bounds__(256) fs_clahe_map(const float *in, float *out, int W, int H, int TX, int TY, int bh,
-                                                    int stage_rows, const float *__restrict__ luts) {
-	extern __shared__ __align__(16) float ch_fsmem[];
-	const int f = blockIdx.y, r0 = blockIdx.x * bh, r1 = (r0 + bh < H) ? r0 + bh : H;
-	float *s_lut = ch_fsmem, *s_cw = s_lut + (size_t) stage_rows * TX * CH_BINS, *s_rw = s_cw + W;
-	uchar2 *s_cj = reinterpret_cast<uchar2 *>(s_rw + bh), *s_rj = s_cj + W;
-	for (int x = threadIdx.x; x < W; x += blockDim.x) { uchar2 j; ch_axis(x, W, TX, &j.x, &j.y, &s_cw[x]); s_cj[x] = j; }
-	for (int y = threadIdx.x; y < r1 - r0; y += blockDim.x) { uchar2 j; ch_axis(r0 + y, H, TY, &j.x, &j.y, &s_rw[y]); s_rj[y] = j; }
-	__syncthreads();
-	const int i_lo = s_rj[0].x, i_hi = s_rj[r1 - r0 - 1].y, tile_row = TX * CH_BINS;
-	const float *g = luts + (size_t) f * TY * tile_row;
-	const float *L = g;
-	int base_row = 0;
-	if (i_hi - i_lo + 1 <= stage_rows) {                 // block-uniform
-		const float4 *s4 = reinterpret_cast<const float4 *>(g + (size_t) i_lo * tile_row);
-		float4 *d4 = reinterpret_cast<float4 *>(s_lut);
-		for (int k = threadIdx.x; k < (i_hi - i_lo + 1) * tile_row / 4; k += blockDim.x) d4[k] = __ldg(s4 + k);
-		__syncthreads();
-		L = s_lut; base_row = i_lo;
-	}
-	auto map = [&](float v, int x, int yy) -> float {
-		if (!ch_valid(v)) return v;
-		const int bin = ch_bin(v);
-		const uchar2 cj = s_cj[x], rj = s_rj[yy];
-		const float wx = s_cw[x], wy = s_rw[yy];
-		const float *l0 = L + (rj.x - base_row) * tile_row + bin, *l1 = L + (rj.y - base_row) * tile_row + bin;
-		const float a = l0[cj.x * CH_BINS], b = l0[cj.y * CH_BINS], c = l1[cj.x * CH_BINS], d = l1[cj.y * CH_BINS];
-		const float top = __fadd_rn(a, __fmul_rn(wx, __fsub_rn(b, a)));
-		const float bot = __fadd_rn(c, __fmul_rn(wx, __fsub_rn(d, c)));
-		return __fadd_rn(top, __fmul_rn(wy, __fsub_rn(bot, top)));
-	};
-	const size_t off = (size_t) f * W * H + (size_t) r0 * W;
-	const float *src = in + off;
-	float *dst = out + off;
-	const unsigned uw = (unsigned) W, count = (unsigned) ((r1 - r0) * W);
-	if (!VEC) {
-		for (unsigned q = threadIdx.x; q < count; q += blockDim.x) dst[q] = map(src[q], (int) (q % uw), (int) (q / uw));
-		return;
-	}
-	const ChBand band(src, count);
-	if (threadIdx.x < band.head) { const unsigned q = threadIdx.x; dst[q] = map(src[q], (int) (q % uw), (int) (q / uw)); }
-	if (threadIdx.x < band.n - band.tail0) {
-		const unsigned q = (unsigned) (band.tail0 + threadIdx.x);
-		dst[q] = map(src[q], (int) (q % uw), (int) (q / uw));
-	}
-	const float4 *src4 = reinterpret_cast<const float4 *>(src + band.head);
-	float4 *dst4 = reinterpret_cast<float4 *>(dst + band.head);
-	auto map4 = [&](float4 v, size_t k) {
-		const unsigned q = (unsigned) (band.head + 4 * k);
-		int x = (int) (q % uw), y = (int) (q / uw);
-		v.x = map(v.x, x, y); if (++x == W) { x = 0; y++; }
-		v.y = map(v.y, x, y); if (++x == W) { x = 0; y++; }
-		v.z = map(v.z, x, y); if (++x == W) { x = 0; y++; }
-		v.w = map(v.w, x, y);
-		dst4[k] = v;
-	};
-	// two float4s per thread and iteration, both loaded before either is stored (in place, the stores could alias later loads)
-	for (size_t k = threadIdx.x; k < band.nbody; k += 2 * blockDim.x) {
-		const size_t k2 = k + blockDim.x;
-		const float4 v = src4[k], u = (k2 < band.nbody) ? src4[k2] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-		map4(v, k);
-		if (k2 < band.nbody) map4(u, k2);
-	}
-}
-
-// ---------------------------------------------------------------- non-local means (beyond the reference; the definition is in tsdrgpu.h)
-// A CTA of NL_TW x NL_BY threads owns an output tile of NL_TW columns by NL_BY K rows of one frame (frames on grid.y).  Shared
-// memory holds the tile's guide g_c with a fixed halo of R_max + P_max and its (masked value, mask) pairs with a fixed halo of
-// R_max, so the row pitches are constants and every shared load is a register base plus an immediate; only the rows and
-// columns the actual R and P reach are filled.  A thread owns one column and K consecutive rows.  The guide values of its
-// centre patches (K + 2P rows by 2P + 1 columns) stay in registers for all offsets.  Along dx the neighbours' guide values
-// slide through a rotating register window (the dx loop is unrolled by 2P + 1, so the slot of every column is a constant),
-// which takes one new column, K + 2P loads, per offset.  Each offset then costs per pixel one LDS.64 of (v_n, m) and the
-// arithmetic of the definition; the mask multiplies the weight (w m is w or +0, and adding +0 leaves either accumulator as
-// it was, since neither can be -0), so no branch or select depends on the neighbour.
-constexpr int NL_TW = 64, NL_BY = 4;
-constexpr int NL_GH = TSDRGPU_NLM_MAX_R + TSDRGPU_NLM_MAX_P, NL_VH = TSDRGPU_NLM_MAX_R;
-constexpr int NL_GW = NL_TW + 2 * NL_GH, NL_VW = NL_TW + 2 * NL_VH;       // row pitches of the guide and value planes
-template <int K> constexpr size_t nl_smem_bytes() {
-	return sizeof(float) * NL_GW * (NL_BY * K + 2 * NL_GH) + sizeof(float2) * NL_VW * (NL_BY * K + 2 * NL_VH);
-}
-
-template <int P, int K>
-__global__ void __launch_bounds__(NL_TW * NL_BY) fs_nlm(const float *__restrict__ in, float *__restrict__ out, int W, int H,
-                                                       int tiles_x, int R, float inv) {
-	constexpr int TH = NL_BY * K, WN = 2 * P + 1, ROWS = K + 2 * P;
-	extern __shared__ __align__(16) float nl_smem[];
-	float *sG = nl_smem;
-	float2 *sV = reinterpret_cast<float2 *>(nl_smem + NL_GW * (TH + 2 * NL_GH));
-	const int x0 = (int) (blockIdx.x % (unsigned) tiles_x) * NL_TW, y0 = (int) (blockIdx.x / (unsigned) tiles_x) * TH;
-	const int tx = threadIdx.x, ty = threadIdx.y;
-	const float *src = in + (size_t) blockIdx.y * W * H;
-	const int hg = R + P;
-	for (int r = NL_GH - hg + ty; r < NL_GH + TH + hg; r += NL_BY) {
-		const int yy = min(max(y0 - NL_GH + r, 0), H - 1);
-		const float *row = src + (size_t) yy * W;
-		for (int c = NL_GH - hg + tx; c < NL_GH + NL_TW + hg; c += NL_TW) {
-			const float v = __ldg(row + min(max(x0 - NL_GH + c, 0), W - 1));
-			sG[r * NL_GW + c] = ch_valid(v) ? fminf(fmaxf(v, 0.0f), 1.0f) : 0.0f;
-		}
-	}
-	for (int r = NL_VH - R + ty; r < NL_VH + TH + R; r += NL_BY) {
-		const int yy = y0 - NL_VH + r;
-		for (int c = NL_VH - R + tx; c < NL_VH + NL_TW + R; c += NL_TW) {
-			const int xx = x0 - NL_VH + c;
-			float2 q = make_float2(0.0f, 0.0f);
-			if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-				const float v = __ldg(src + (size_t) yy * W + xx);
-				if (ch_valid(v)) q = make_float2(v, 1.0f);
-			}
-			sV[r * NL_VW + c] = q;
-		}
-	}
-	__syncthreads();
-	const int x = x0 + tx, yt = y0 + ty * K;
-	if (x >= W || yt >= H) return;
-	const float *cg = sG + (NL_GH + ty * K - P) * NL_GW + NL_GH + tx - P;     // top-left of the thread's centre patches
-	float cw[ROWS][WN];
-#pragma unroll
-	for (int j = 0; j < ROWS; j++)
-#pragma unroll
-		for (int c = 0; c < WN; c++) cw[j][c] = cg[j * NL_GW + c];
-	float aw[K], av[K];
-#pragma unroll
-	for (int i = 0; i < K; i++) { aw[i] = 0.0f; av[i] = 0.0f; }
-	for (int dy = -R; dy <= R; dy++) {
-		const float *nb = cg + dy * NL_GW - R;                          // neighbour window of dx = -R, column 0
-		const float2 *vb = sV + (NL_VH + ty * K + dy) * NL_VW + NL_VH + tx - R;
-		float nw[ROWS][WN];
-#pragma unroll
-		for (int j = 0; j < ROWS; j++)
-#pragma unroll
-			for (int c = 0; c < WN - 1; c++) nw[j][c] = nb[j * NL_GW + c];
-		for (int kb = 0; kb <= 2 * R; kb += WN) {
-#pragma unroll
-			for (int r = 0; r < WN; r++) {
-				const int k = kb + r;                                   // dx = k - R
-				if (k > 2 * R) break;
-#pragma unroll
-				for (int j = 0; j < ROWS; j++) nw[j][(r + WN - 1) % WN] = nb[j * NL_GW + k + WN - 1];
-				float s[ROWS];
-#pragma unroll
-				for (int j = 0; j < ROWS; j++) {
-#pragma unroll
-					for (int c = 0; c < WN; c++) {
-						const float d = __fsub_rn(cw[j][c], nw[j][(r + c) % WN]);
-						const float e = __fmul_rn(d, d);
-						s[j] = (c == 0) ? e : __fadd_rn(s[j], e);
-					}
-				}
-#pragma unroll
-				for (int i = 0; i < K; i++) {
-					float d = s[i];
-#pragma unroll
-					for (int p = 1; p < WN; p++) d = __fadd_rn(d, s[i + p]);
-					const float u = __fsub_rn(1.0f, fminf(__fmul_rn(d, inv), 1.0f));
-					const float2 q = vb[i * NL_VW + k];
-					const float wm = __fmul_rn(__fmul_rn(u, u), q.y);
-					aw[i] = __fadd_rn(aw[i], wm);
-					av[i] = __fadd_rn(av[i], __fmul_rn(wm, q.x));
-				}
-			}
-		}
-	}
-#pragma unroll
-	for (int i = 0; i < K; i++) {
-		if (yt + i >= H) break;
-		const size_t o = (size_t) (yt + i) * W + x;
-		const float v = __ldg(src + o);
-		out[(size_t) blockIdx.y * W * H + o] = ch_valid(v) ? __fdiv_rn(av[i], aw[i]) : v;
-	}
-}
-
 }  // namespace
+
+int fs_copy_async(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, size_t total) {
+	KL(ctx, "fs_copy", stream, fs_copy<<<grid_for(total, ctx->sm_count), 256, 0, stream>>>(in, out, total));
+	return TSDRGPU_OK;
+}
 
 // -----------------------------------------------------------------------------------------------------------------
 struct tsdrgpu_framestage {
@@ -1669,10 +1352,7 @@ struct tsdrgpu_framestage {
 	float *d_pmin, *d_pmax; double *d_psum, *d_psq, *d_plin; FrameParams *d_params; int batch_cap;
 	int ag_mode, ag_ppm;                         // tsdrgpu_framestage_set_autogain (kept across reset)
 	unsigned *d_sel_hist; SelState *d_sel; float2 *d_levels;     // clip-mode selection, batch_cap frames
-	int ct_mode, ct_clip, ct_tx, ct_ty;          // tsdrgpu_framestage_set_contrast (kept across reset)
-	unsigned *d_clahe; size_t clahe_cap;         // CLAHE histograms / LUTs of one pass, words
-	int nl_mode, nl_h, nl_r, nl_p;               // tsdrgpu_framestage_set_denoise (kept across reset)
-	float *d_nlm; size_t nlm_cap;                // NLM output of a batch, only ever touched on the stream the output becomes valid on
+	EnhanceState enh;                            // tsdrgpu_framestage_set_contrast / _set_denoise (kept across reset)
 	tsdrgpu_frame_result_t *d_results[2];
 	double *d_chain;
 	int *d_resume;                               // first frame of the batch fs_sync_walk could not serve from the tables
@@ -1684,32 +1364,6 @@ struct tsdrgpu_framestage {
 	cudaEvent_t ev_done[2];                      // side: sync + emit of this phase done -> buffers of the phase are free
 	CollapseMaps collapse_maps[4];               // fs_collapse_tiles' tensor maps of the buffers collapsed last (d_t2[0/1], d_t1)
 };
-
-// CLAHE: effective tile grid, frames per pass and the words one pass of the histogram buffer needs
-struct ChGeom { int tx, ty, fpp; size_t words; };
-static ChGeom ch_geom(const tsdrgpu_framestage *fs, int nframes, int w, int h) {
-	ChGeom g;
-	g.tx = fs->ct_tx < w ? fs->ct_tx : w; g.ty = fs->ct_ty < h ? fs->ct_ty : h;
-	const size_t per_frame = (size_t) g.tx * g.ty * CH_BINS;
-	size_t fpp = CH_PASS_WORDS / per_frame;
-	if (fpp > (size_t) nframes) fpp = (size_t) nframes;
-	if (fpp > 65535) fpp = 65535;
-	g.fpp = fpp ? (int) fpp : 1;
-	g.words = (size_t) g.fpp * per_frame;
-	return g;
-}
-
-static int fs_reserve_clahe(tsdrgpu_framestage *fs, int nframes, int w, int h) {
-	if (fs->ct_mode != TSDRGPU_CONTRAST_CLAHE) return TSDRGPU_OK;
-	const size_t need = ch_geom(fs, nframes, w, h).words;
-	if (fs->clahe_cap < need) {
-		CU_TRY(fs->ctx, cudaDeviceSynchronize());
-		if (fs->d_clahe) CU_TRY(fs->ctx, cudaFree(fs->d_clahe));
-		CU_TRY(fs->ctx, cudaMalloc(&fs->d_clahe, sizeof(unsigned) * need));
-		fs->clahe_cap = need;
-	}
-	return TSDRGPU_OK;
-}
 
 static int fs_reserve(tsdrgpu_framestage *fs, int nframes, size_t n, int w, int h) {
 	tsdrgpu_ctx_t *ctx = fs->ctx;
@@ -1759,71 +1413,7 @@ static int fs_reserve(tsdrgpu_framestage *fs, int nframes, size_t n, int w, int 
 		CU_TRY(ctx, cudaDeviceSynchronize());
 		fs->batch_cap = nframes;
 	}
-	if (fs->nl_mode == TSDRGPU_DENOISE_NLM && fs->nlm_cap < need) {
-		CU_TRY(ctx, cudaDeviceSynchronize());
-		if (fs->d_nlm) CU_TRY(ctx, cudaFree(fs->d_nlm));
-		CU_TRY(ctx, cudaMalloc(&fs->d_nlm, sizeof(float) * need));
-		fs->nlm_cap = need;
-	}
-	return fs_reserve_clahe(fs, nframes, w, h);
-}
-
-template <int P, int K>
-static int nl_launch(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h, int r,
-                     float inv) {
-	const int tiles_x = (w + NL_TW - 1) / NL_TW, tiles_y = (h + NL_BY * K - 1) / (NL_BY * K);
-	const size_t smem = nl_smem_bytes<K>(), n = (size_t) w * h;
-	CU_TRY(ctx, cudaFuncSetAttribute(fs_nlm<P, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-	for (int f0 = 0; f0 < nframes; f0 += 65535) {
-		const int nf = (nframes - f0 < 65535) ? nframes - f0 : 65535;
-		KL(ctx, "fs_nlm", stream, (fs_nlm<P, K><<<dim3((unsigned) (tiles_x * tiles_y), (unsigned) nf), dim3(NL_TW, NL_BY), smem, stream>>>(
-			in + f0 * n, out + f0 * n, w, h, tiles_x, r, inv)));
-	}
-	return TSDRGPU_OK;
-}
-
-// non-local means of nframes frames of w x h, in -> out (no overlap), on `stream`
-static int fs_nlm_batch(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h, int h_milli,
-                        int r, int p) {
-	const float inv = (float) (1e6 / (4.0 * (double) h_milli * (double) h_milli * (double) ((2 * p + 1) * (2 * p + 1))));
-	if (p == 1) return nl_launch<1, 8>(ctx, stream, in, out, nframes, w, h, r, inv);
-	if (p == 2) return nl_launch<2, 6>(ctx, stream, in, out, nframes, w, h, r, inv);
-	return nl_launch<3, 4>(ctx, stream, in, out, nframes, w, h, r, inv);
-}
-
-// CLAHE of nframes frames of w x h, in -> out (in == out allowed), on `stream`; per pass: zero, histograms, LUTs, mapping
-static int fs_clahe_batch(tsdrgpu_framestage *fs, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h) {
-	tsdrgpu_ctx_t *ctx = fs->ctx;
-	const ChGeom g = ch_geom(fs, nframes, w, h);
-	const size_t n = (size_t) w * h;
-	const int target = ctx->sm_count * 4;                // histogram CTAs per launch: about four per SM over the pass
-	const size_t hist_smem = sizeof(unsigned) * g.tx * CH_BINS + (size_t) ((w + 3) & ~3);
-	const int stage_rows = (3 * g.tx * CH_BINS * (int) sizeof(float) <= CH_STAGE_BYTES) ? 3 : 0;
-	const bool vec = ((reinterpret_cast<unsigned long long>(in) ^ reinterpret_cast<unsigned long long>(out)) & 15ull) == 0;
-	CU_TRY(ctx, cudaFuncSetAttribute(fs_clahe_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) hist_smem));
-	for (int f0 = 0; f0 < nframes; f0 += g.fpp) {
-		const int nf = (nframes - f0 < g.fpp) ? nframes - f0 : g.fpp;
-		CU_TRY(ctx, cudaMemsetAsync(fs->d_clahe, 0, sizeof(unsigned) * nf * g.tx * g.ty * CH_BINS, stream));
-		int parts = (target + nf * g.ty - 1) / (nf * g.ty);
-		if (parts > h / g.ty) parts = h / g.ty;          // every part keeps at least one row
-		if (parts < 1) parts = 1;
-		KL(ctx, "fs_clahe_hist", stream, fs_clahe_hist<<<dim3((unsigned) (g.ty * parts), nf), 256, hist_smem, stream>>>(in + f0 * n, w, h, g.tx, g.ty, parts, fs->d_clahe));
-		KL(ctx, "fs_clahe_lut", stream, fs_clahe_lut<<<dim3((unsigned) (g.tx * g.ty), nf), CH_BINS, 0, stream>>>(fs->d_clahe, fs->ct_clip));
-		int bands = (2 * target + nf - 1) / nf;          // mapping CTAs: about eight per SM
-		if (bands > h) bands = h;
-		const int bh = (h + bands - 1) / bands;
-		bands = (h + bh - 1) / bh;
-		const size_t map_smem = sizeof(float) * ((size_t) stage_rows * g.tx * CH_BINS + w + bh) + sizeof(uchar2) * ((size_t) w + bh);
-		const float *luts = reinterpret_cast<const float *>(fs->d_clahe);
-		if (vec) {
-			CU_TRY(ctx, cudaFuncSetAttribute(fs_clahe_map<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) map_smem));
-			KL(ctx, "fs_clahe_map", stream, fs_clahe_map<true><<<dim3((unsigned) bands, nf), 256, map_smem, stream>>>(in + f0 * n, out + f0 * n, w, h, g.tx, g.ty, bh, stage_rows, luts));
-		} else {
-			CU_TRY(ctx, cudaFuncSetAttribute(fs_clahe_map<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) map_smem));
-			KL(ctx, "fs_clahe_map", stream, fs_clahe_map<false><<<dim3((unsigned) bands, nf), 256, map_smem, stream>>>(in + f0 * n, out + f0 * n, w, h, g.tx, g.ty, bh, stage_rows, luts));
-		}
-	}
-	return TSDRGPU_OK;
+	return enhance_reserve(ctx, &fs->enh, nframes, w, h);
 }
 
 // clip mode's levels of a batch into d_levels (and, with snr, the per-chunk sums into d_psum): three radix-select rounds
@@ -1872,8 +1462,6 @@ int tsdrgpu_framestage_create(tsdrgpu_ctx_t *ctx, tsdrgpu_framestage_t **out) {
 	tsdrgpu_framestage *fs = new tsdrgpu_framestage();
 	memset(fs, 0, sizeof(*fs));
 	fs->ctx = ctx;
-	fs->ct_tx = fs->ct_ty = 8; fs->ct_clip = 200;
-	fs->nl_h = 100; fs->nl_r = 5; fs->nl_p = 1;
 	tsdrgpu_gauss_taps(fs->taps);
 	CU_TRY(ctx, cudaMalloc(&fs->d_state, sizeof(SyncState)));
 	CU_TRY(ctx, cudaMalloc(&fs->d_chain, sizeof(double) * 10 * FS_MAX_STRIP));
@@ -1898,9 +1486,9 @@ void tsdrgpu_framestage_destroy(tsdrgpu_framestage_t *fs) {
 	cudaDeviceSynchronize();
 	void *ptrs[] = {fs->d_screen, fs->d_state, fs->d_t1, fs->d_t2[0], fs->d_t2[1], fs->d_wstrips[0], fs->d_wstrips[1], fs->d_hstrips[0],
 	                fs->d_hstrips[1], fs->d_pmin, fs->d_pmax, fs->d_psum, fs->d_psq, fs->d_plin, fs->d_params, fs->d_results[0],
-	                fs->d_results[1], fs->d_chain, fs->d_prep, fs->d_resume, fs->d_sel_hist, fs->d_sel, fs->d_levels, fs->d_clahe,
-	                fs->d_nlm};
+	                fs->d_results[1], fs->d_chain, fs->d_prep, fs->d_resume, fs->d_sel_hist, fs->d_sel, fs->d_levels};
 	for (void *p : ptrs) if (p) cudaFree(p);
+	enhance_free(&fs->enh);
 	cudaStreamDestroy(fs->s_side);
 	for (int i = 0; i < 2; i++) { cudaEventDestroy(fs->ev_ready[i]); cudaEventDestroy(fs->ev_done[i]); }
 	delete fs;
@@ -1921,112 +1509,25 @@ int tsdrgpu_framestage_reset(tsdrgpu_framestage_t *fs, void *stream) {
 
 int tsdrgpu_framestage_set_autogain(tsdrgpu_framestage_t *fs, int mode, int ppm) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, fs != NULL);
-	ARG_TRY(fs->ctx, (mode == TSDRGPU_AG_MINMAX || mode == TSDRGPU_AG_CLIP) && ppm >= 0 && ppm <= TSDRGPU_AG_MAX_PPM);
+	ARG_TRY(fs->ctx, autogain_ok(mode, ppm));
 	fs->ag_mode = mode; fs->ag_ppm = ppm;
 	return TSDRGPU_OK;
 }
 
-static bool ch_params_ok(int mode, int clip_centi, int tx, int ty) {
-	return mode == TSDRGPU_CONTRAST_OFF || (mode == TSDRGPU_CONTRAST_CLAHE && clip_centi >= TSDRGPU_CLAHE_MIN_CLIP &&
-	       clip_centi <= TSDRGPU_CLAHE_MAX_CLIP && tx >= 1 && tx <= TSDRGPU_CLAHE_MAX_TILES && ty >= 1 && ty <= TSDRGPU_CLAHE_MAX_TILES);
-}
-
 int tsdrgpu_framestage_set_contrast(tsdrgpu_framestage_t *fs, int mode, int clip_centi, int tx, int ty) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, fs != NULL);
-	ARG_TRY(fs->ctx, ch_params_ok(mode, clip_centi, tx, ty));
-	fs->ct_mode = mode;
-	if (mode == TSDRGPU_CONTRAST_CLAHE) { fs->ct_clip = clip_centi; fs->ct_tx = tx; fs->ct_ty = ty; }
+	ARG_TRY(fs->ctx, contrast_ok(mode, clip_centi, tx, ty));
+	fs->enh.contrast = mode;
+	if (mode == TSDRGPU_CONTRAST_CLAHE) { fs->enh.clip_centi = clip_centi; fs->enh.tx = tx; fs->enh.ty = ty; }
 	return TSDRGPU_OK;
-}
-
-static bool nl_params_ok(int mode, int h_milli, int r, int p) {
-	return mode == TSDRGPU_DENOISE_OFF || (mode == TSDRGPU_DENOISE_NLM && h_milli >= 1 && h_milli <= TSDRGPU_NLM_MAX_H && r >= 1 &&
-	       r <= TSDRGPU_NLM_MAX_R && p >= 1 && p <= TSDRGPU_NLM_MAX_P);
 }
 
 int tsdrgpu_framestage_set_denoise(tsdrgpu_framestage_t *fs, int mode, int h_milli, int r, int p) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, fs != NULL);
-	ARG_TRY(fs->ctx, nl_params_ok(mode, h_milli, r, p));
-	fs->nl_mode = mode;
-	if (mode == TSDRGPU_DENOISE_NLM) { fs->nl_h = h_milli; fs->nl_r = r; fs->nl_p = p; }
+	ARG_TRY(fs->ctx, denoise_ok(mode, h_milli, r, p));
+	fs->enh.denoise = mode;
+	if (mode == TSDRGPU_DENOISE_NLM) { fs->enh.h_milli = h_milli; fs->enh.r = r; fs->enh.p = p; }
 	return TSDRGPU_OK;
-}
-
-// one to six decimal digits -> their value, with *end past them; -1 for none or more than six
-static int ch_digits(const char *c, const char **end) {
-	int v = 0, d = 0;
-	while (*c >= '0' && *c <= '9' && d < 7) { v = 10 * v + (*c - '0'); c++; d++; }
-	*end = c;
-	return (d == 0 || d == 7) ? -1 : v;
-}
-
-int tsdrgpu_contrast_parse(const char *spec, int *mode, int *clip_centi, int *tx, int *ty) {
-	if (!spec || !mode || !clip_centi || !tx || !ty) return TSDRGPU_EINVAL;
-	if (strcmp(spec, "off") == 0) { *mode = TSDRGPU_CONTRAST_OFF; *clip_centi = 0; *tx = 0; *ty = 0; return TSDRGPU_OK; }
-	if (strncmp(spec, "clahe:", 6) != 0) return TSDRGPU_EINVAL;
-	const char *c = spec + 6;
-	const int whole = ch_digits(c, &c);
-	if (whole < 0) return TSDRGPU_EINVAL;
-	int centi = whole * 100;
-	if (*c == '.') {
-		const char *f = ++c;
-		const int frac = ch_digits(f, &c);
-		if (frac < 0 || c - f > 2) return TSDRGPU_EINVAL;
-		centi += (c - f == 1) ? 10 * frac : frac;
-	}
-	int x = 8, y = 8;
-	if (*c == ':') {
-		x = ch_digits(c + 1, &c);
-		if (x < 0 || *c != 'x') return TSDRGPU_EINVAL;
-		y = ch_digits(c + 1, &c);
-		if (y < 0) return TSDRGPU_EINVAL;
-	}
-	if (*c || !ch_params_ok(TSDRGPU_CONTRAST_CLAHE, centi, x, y)) return TSDRGPU_EINVAL;
-	*mode = TSDRGPU_CONTRAST_CLAHE; *clip_centi = centi; *tx = x; *ty = y;
-	return TSDRGPU_OK;
-}
-
-int tsdrgpu_denoise_parse(const char *spec, int *mode, int *h_milli, int *r, int *p) {
-	if (!spec || !mode || !h_milli || !r || !p) return TSDRGPU_EINVAL;
-	if (strcmp(spec, "off") == 0) { *mode = TSDRGPU_DENOISE_OFF; *h_milli = 0; *r = 0; *p = 0; return TSDRGPU_OK; }
-	if (strncmp(spec, "nlm:", 4) != 0) return TSDRGPU_EINVAL;
-	const char *c = spec + 4;
-	const int whole = ch_digits(c, &c);
-	if (whole < 0 || whole > 1) return TSDRGPU_EINVAL;
-	int milli = whole * 1000;
-	if (*c == '.') {
-		const char *f = ++c;
-		const int frac = ch_digits(f, &c);
-		if (frac < 0 || c - f > 3) return TSDRGPU_EINVAL;
-		milli += (c - f == 1) ? 100 * frac : (c - f == 2) ? 10 * frac : frac;
-	}
-	int rr = 5, pp = 1;
-	if (*c == ':') {
-		rr = ch_digits(c + 1, &c);
-		if (rr < 0 || *c != ':') return TSDRGPU_EINVAL;
-		pp = ch_digits(c + 1, &c);
-		if (pp < 0) return TSDRGPU_EINVAL;
-	}
-	if (*c || !nl_params_ok(TSDRGPU_DENOISE_NLM, milli, rr, pp)) return TSDRGPU_EINVAL;
-	*mode = TSDRGPU_DENOISE_NLM; *h_milli = milli; *r = rr; *p = pp;
-	return TSDRGPU_OK;
-}
-
-int tsdrgpu_autogain_ppm(const char *percent) {
-	if (!percent) return -1;
-	const char *c = percent;
-	int digits = 0;
-	while (*c >= '0' && *c <= '9') { c++; digits++; }
-	if (digits == 0) return -1;
-	if (*c == '.') {
-		c++; digits = 0;
-		while (*c >= '0' && *c <= '9') { c++; digits++; }
-		if (digits == 0) return -1;
-	}
-	if (*c) return -1;
-	const double v = strtod(percent, NULL);          // a plain decimal: correctly rounded, as Python's float()
-	if (!(v <= 25.0)) return -1;
-	return (int) floor(v * 1e4 + 0.5);
 }
 
 int tsdrgpu_framestage_set_overlap(tsdrgpu_framestage_t *fs, int on) {
@@ -2133,14 +1634,10 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 			KL(ctx, "fs_greenlines", s2, fs_greenlines<<<dim3(8, nframes), 256, 0, s2>>>(src, w, h, d_results));
 			*result = src;
 		} else if (greenlines) {
-			KL(ctx, "fs_copy", s2, fs_copy<<<grid_for(total, ctx->sm_count), 256, 0, s2>>>(src, dst, total));
+			if ((rc = fs_copy_async(ctx, s2, src, dst, total))) return rc;
 			KL(ctx, "fs_greenlines", s2, fs_greenlines<<<dim3(8, nframes), 256, 0, s2>>>(dst, w, h, d_results));
 			*result = dst;
 		} else *result = src;
-		return TSDRGPU_OK;
-	};
-	auto copy_to_out = [&](const float *src, cudaStream_t s2) -> int {
-		if (src != d_out) KL(ctx, "fs_copy", s2, fs_copy<<<grid_for(total, ctx->sm_count), 256, 0, s2>>>(src, d_out, total));
 		return TSDRGPU_OK;
 	};
 	float *res = NULL;
@@ -2171,13 +1668,13 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 		if (aap) {
 			if ((rc = fs_autogain_batch(fs, stream, res, d_out, nframes, n, lowpasscoeff, snr))) return rc;
 			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
-		} else if ((rc = copy_to_out(res, tail))) return rc;
+		} else if (res != d_out && (rc = fs_copy_async(ctx, tail, res, d_out, total))) return rc;
 	} else {                                             // dsp.c:214-226
 		float *work = fs->d_t1;
 		if (!aap) {
 			if ((rc = fs_autogain_batch(fs, stream, d_in, fs->d_t1, nframes, n, lowpasscoeff, snr))) return rc;
 			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
-		} else KL(ctx, "fs_copy", stream, fs_copy<<<grid_for(total, ctx->sm_count), 256, 0, stream>>>(d_in, fs->d_t1, total));
+		} else if ((rc = fs_copy_async(ctx, stream, d_in, fs->d_t1, total))) return rc;
 		if ((rc = collapse_sync(work, stream))) return rc;
 		if ((rc = emit(work, T2, (motionblur == 0.0f) && !superres, true, &res, stream))) return rc;
 		float *lp_out = aap ? ((res == fs->d_t1) ? T2 : fs->d_t1) : d_out;
@@ -2187,15 +1684,8 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
 		}
 	}
-	// NLM, then CLAHE, on the frames as delivered, after every branch's last step; nothing either does feeds back.  NLM cannot
-	// run in place: it writes the frame stage's own scratch buffer, which only `tail` touches (in overlap mode the main stream
-	// is already filling d_t1 and the other phase's T2 with the next batch), and CLAHE or one copy brings the frames back.
-	const bool clahe = fs->ct_mode == TSDRGPU_CONTRAST_CLAHE;
-	if (fs->nl_mode == TSDRGPU_DENOISE_NLM) {
-		if ((rc = fs_nlm_batch(ctx, tail, d_out, fs->d_nlm, nframes, w, h, fs->nl_h, fs->nl_r, fs->nl_p))) return rc;
-		if (clahe) { if ((rc = fs_clahe_batch(fs, tail, fs->d_nlm, d_out, nframes, w, h))) return rc; }
-		else KL(ctx, "fs_copy", tail, fs_copy<<<grid_for(total, ctx->sm_count), 256, 0, tail>>>(fs->d_nlm, d_out, total));
-	} else if (clahe && (rc = fs_clahe_batch(fs, tail, d_out, d_out, nframes, w, h))) return rc;
+	// NLM, then CLAHE, on the frames as delivered, after every branch's last step; nothing either does feeds back
+	if ((rc = enhance_run(ctx, &fs->enh, tail, d_out, nframes, w, h))) return rc;
 	if (h_results) CU_TRY(ctx, cudaMemcpyAsync(h_results, d_results, sizeof(tsdrgpu_frame_result_t) * nframes, cudaMemcpyDeviceToHost, tail));
 	if (overlapped) {
 		CU_TRY(ctx, cudaEventRecord(fs->ev_done[ph], fs->s_side));
@@ -2250,7 +1740,7 @@ int tsdrgpu_frame_levels(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_frame
 	BIND(ctx);
 	if (nframes == 0) return TSDRGPU_OK;
 	ARG_TRY(ctx, d_frames && h_lo && h_hi && n > 0 && n <= TSDRGPU_MAX_FRAME_PIXELS && nframes > 0 && nframes <= 65535);
-	ARG_TRY(ctx, ppm >= 0 && ppm <= TSDRGPU_AG_MAX_PPM && (((uintptr_t) d_frames) & 3) == 0);
+	ARG_TRY(ctx, autogain_ok(TSDRGPU_AG_CLIP, ppm) && (((uintptr_t) d_frames) & 3) == 0);
 	cudaStream_t stream = (cudaStream_t) stream_;
 	tsdrgpu_framestage_t *fs;
 	int rc = tsdrgpu_framestage_create(ctx, &fs);
@@ -2267,40 +1757,6 @@ int tsdrgpu_frame_levels(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_frame
 		free(lv); free(st);
 	}
 	tsdrgpu_framestage_destroy(fs);
-	return rc;
-}
-
-int tsdrgpu_clahe(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_in, float *d_out, int w, int h, int nframes, int clip_centi,
-                  int tx, int ty) {
-	BIND(ctx);
-	if (nframes == 0) return TSDRGPU_OK;
-	ARG_TRY(ctx, d_in && d_out && nframes > 0 && w > 0 && h > 0 && w <= FS_MAX_STRIP && h <= FS_MAX_STRIP);
-	ARG_TRY(ctx, (size_t) w * h <= TSDRGPU_MAX_FRAME_PIXELS && ((((uintptr_t) d_in) | ((uintptr_t) d_out)) & 3) == 0);
-	ARG_TRY(ctx, ch_params_ok(TSDRGPU_CONTRAST_CLAHE, clip_centi, tx, ty));
-	cudaStream_t stream = (cudaStream_t) stream_;
-	tsdrgpu_framestage_t *fs;
-	int rc = tsdrgpu_framestage_create(ctx, &fs);
-	if (rc) return rc;
-	if (!(rc = tsdrgpu_framestage_set_contrast(fs, TSDRGPU_CONTRAST_CLAHE, clip_centi, tx, ty)) && !(rc = fs_reserve_clahe(fs, nframes, w, h)) &&
-	    !(rc = fs_clahe_batch(fs, stream, d_in, d_out, nframes, w, h))) {
-		cudaError_t e = cudaStreamSynchronize(stream);
-		if (e != cudaSuccess) rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "tsdrgpu_clahe", e, __FILE__, __LINE__);
-	}
-	tsdrgpu_framestage_destroy(fs);
-	return rc;
-}
-
-int tsdrgpu_nlm(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_in, float *d_out, int w, int h, int nframes, int h_milli, int r,
-                int p) {
-	BIND(ctx);
-	if (nframes == 0) return TSDRGPU_OK;
-	ARG_TRY(ctx, d_in && d_out && nframes > 0 && w > 0 && h > 0 && (size_t) w * h <= TSDRGPU_MAX_FRAME_PIXELS);
-	ARG_TRY(ctx, ((((uintptr_t) d_in) | ((uintptr_t) d_out)) & 3) == 0 && nl_params_ok(TSDRGPU_DENOISE_NLM, h_milli, r, p));
-	const uintptr_t bytes = (uintptr_t) sizeof(float) * w * h * nframes;
-	ARG_TRY(ctx, (uintptr_t) d_out >= (uintptr_t) d_in + bytes || (uintptr_t) d_in >= (uintptr_t) d_out + bytes);
-	cudaStream_t stream = (cudaStream_t) stream_;
-	int rc = fs_nlm_batch(ctx, stream, d_in, d_out, nframes, w, h, h_milli, r, p);
-	if (rc == TSDRGPU_OK) CU_TRY(ctx, cudaStreamSynchronize(stream));
 	return rc;
 }
 

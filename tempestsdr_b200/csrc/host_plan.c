@@ -3,6 +3,7 @@
  * operation order so the device kernels receive bit-identical parameters. */
 #include "host_plan.h"
 #include <math.h>
+#include <stdlib.h>
 #include <string.h>
 
 uint64_t tsdrgpu_plan_resample(double *offset, const uint32_t *sizes, uint32_t uniform, uint32_t nblocks,
@@ -146,6 +147,85 @@ int tsdrgpu_channel_parse(const char *spec, tsdrgpu_channel_t *out) {
 	if (*c || !channel_valid(&s)) return TSDRGPU_EINVAL;
 	*out = s;
 	return TSDRGPU_OK;
+}
+
+/* ---- auto-gain, contrast and denoise options (definitions in tsdrgpu.h) */
+int autogain_ok(int mode, int ppm) {
+	return (mode == TSDRGPU_AG_MINMAX || mode == TSDRGPU_AG_CLIP) && ppm >= 0 && ppm <= TSDRGPU_AG_MAX_PPM;
+}
+
+int contrast_ok(int mode, int clip_centi, int tx, int ty) {
+	return mode == TSDRGPU_CONTRAST_OFF || (mode == TSDRGPU_CONTRAST_CLAHE && clip_centi >= TSDRGPU_CLAHE_MIN_CLIP &&
+	       clip_centi <= TSDRGPU_CLAHE_MAX_CLIP && tx >= 1 && tx <= TSDRGPU_CLAHE_MAX_TILES && ty >= 1 && ty <= TSDRGPU_CLAHE_MAX_TILES);
+}
+
+int denoise_ok(int mode, int h_milli, int r, int p) {
+	return mode == TSDRGPU_DENOISE_OFF || (mode == TSDRGPU_DENOISE_NLM && h_milli >= 1 && h_milli <= TSDRGPU_NLM_MAX_H && r >= 1 &&
+	       r <= TSDRGPU_NLM_MAX_R && p >= 1 && p <= TSDRGPU_NLM_MAX_P);
+}
+
+/* one to six decimal digits -> their value, *c moved past them; -1 for none or more than six */
+static int option_digits(const char **c) {
+	int v = 0, d = 0;
+	while (**c >= '0' && **c <= '9' && d < 7) { v = 10 * v + (**c - '0'); (*c)++; d++; }
+	return (d == 0 || d == 7) ? -1 : v;
+}
+
+/* the contrast and denoise spellings: "off" -> 0 with v = {0, 0, 0}; "<prefix><x>" or "<prefix><x>:<a><sep><b>" -> 1 with
+ * v = {x, a, b}, a and b defaulting to da and db.  x = a whole part of one to six digits, then optionally '.' and one to k
+ * digits, read as the integer x 10^k.  -1 if malformed; the ranges are the caller's. */
+static int option_parse(const char *spec, const char *prefix, int k, char sep, int da, int db, int v[3]) {
+	if (strcmp(spec, "off") == 0) { v[0] = v[1] = v[2] = 0; return 0; }
+	const size_t np = strlen(prefix);
+	if (strncmp(spec, prefix, np) != 0) return -1;
+	const char *c = spec + np;
+	if ((v[0] = option_digits(&c)) < 0) return -1;
+	for (int i = 0; i < k; i++) v[0] *= 10;
+	if (*c == '.') {
+		const char *f = ++c;
+		int frac = option_digits(&c);
+		const int nd = (int) (c - f);
+		if (frac < 0 || nd > k) return -1;
+		for (int i = nd; i < k; i++) frac *= 10;
+		v[0] += frac;
+	}
+	v[1] = da; v[2] = db;
+	if (*c == ':') {
+		c++; v[1] = option_digits(&c);
+		if (*c != sep) return -1;
+		c++; v[2] = option_digits(&c);
+	}
+	return *c ? -1 : 1;
+}
+
+int tsdrgpu_contrast_parse(const char *spec, int *mode, int *clip_centi, int *tx, int *ty) {
+	int v[3], on;
+	if (!spec || !mode || !clip_centi || !tx || !ty || (on = option_parse(spec, "clahe:", 2, 'x', 8, 8, v)) < 0) return TSDRGPU_EINVAL;
+	const int m = on ? TSDRGPU_CONTRAST_CLAHE : TSDRGPU_CONTRAST_OFF;
+	if (!contrast_ok(m, v[0], v[1], v[2])) return TSDRGPU_EINVAL;
+	*mode = m; *clip_centi = v[0]; *tx = v[1]; *ty = v[2];
+	return TSDRGPU_OK;
+}
+
+int tsdrgpu_denoise_parse(const char *spec, int *mode, int *h_milli, int *r, int *p) {
+	int v[3], on;
+	if (!spec || !mode || !h_milli || !r || !p || (on = option_parse(spec, "nlm:", 3, ':', 5, 1, v)) < 0) return TSDRGPU_EINVAL;
+	const int m = on ? TSDRGPU_DENOISE_NLM : TSDRGPU_DENOISE_OFF;
+	if (!denoise_ok(m, v[0], v[1], v[2])) return TSDRGPU_EINVAL;
+	*mode = m; *h_milli = v[0]; *r = v[1]; *p = v[2];
+	return TSDRGPU_OK;
+}
+
+/* its own rule, not option_parse's: any number of digits, and the value is rounded from the correctly rounded double */
+int tsdrgpu_autogain_ppm(const char *percent) {
+	if (!percent) return -1;
+	const char *c = percent + strspn(percent, "0123456789");
+	if (c == percent) return -1;
+	if (*c == '.') { const char *f = c + 1; c = f + strspn(f, "0123456789"); if (c == f) return -1; }
+	if (*c) return -1;
+	const double v = strtod(percent, NULL);          /* a plain decimal: correctly rounded, as Python's float() */
+	if (!(v <= 25.0)) return -1;
+	return (int) floor(v * 1e4 + 0.5);
 }
 
 static double clampd(double v, double lo, double hi) { return v < lo ? lo : (v > hi ? hi : v); }

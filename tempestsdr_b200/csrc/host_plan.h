@@ -4,4 +4,14 @@
 #ifndef TSDRGPU_HOST_PLAN_H_
 #define TSDRGPU_HOST_PLAN_H_
 #include "../../include/tsdrgpu.h"
+#ifdef __cplusplus
+extern "C" {
+#endif
+/* internal: 1 when a mode and its parameters are in tsdrgpu.h's ranges (contrast and denoise ignore them when off), else 0 */
+int autogain_ok(int mode, int ppm);
+int contrast_ok(int mode, int clip_centi, int tx, int ty);
+int denoise_ok(int mode, int h_milli, int r, int p);
+#ifdef __cplusplus
+}
+#endif
 #endif

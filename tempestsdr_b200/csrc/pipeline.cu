@@ -18,6 +18,7 @@
 //   * geometry changes made by the PLL take effect at the next batch boundary;
 //   * tsdr_sync offsets are applied between batches of decimator blocks rather than between single blocks.
 #include "common.cuh"
+#include "host_plan.h"
 #include <math.h>
 #include <pthread.h>
 #include <deque>
@@ -726,17 +727,13 @@ int tsdrgpu_pipeline_set_resampler(tsdrgpu_pipeline_t *p, int kernel) {
 	return TSDRGPU_OK;
 }
 int tsdrgpu_pipeline_set_autogain(tsdrgpu_pipeline_t *p, int mode, int ppm) {
-	if (!p || (mode != TSDRGPU_AG_MINMAX && mode != TSDRGPU_AG_CLIP) || ppm < 0 || ppm > TSDRGPU_AG_MAX_PPM) return TSDRGPU_EINVAL;
+	if (!p || !autogain_ok(mode, ppm)) return TSDRGPU_EINVAL;
 	p->ag_ppm = ppm; p->ag_mode = mode;
 	return TSDRGPU_OK;
 }
 int tsdrgpu_pipeline_set_contrast(tsdrgpu_pipeline_t *p, int mode, int clip_centi, int tx, int ty) {
-	if (!p || (mode != TSDRGPU_CONTRAST_OFF && mode != TSDRGPU_CONTRAST_CLAHE)) return TSDRGPU_EINVAL;
-	if (mode == TSDRGPU_CONTRAST_CLAHE) {
-		if (clip_centi < TSDRGPU_CLAHE_MIN_CLIP || clip_centi > TSDRGPU_CLAHE_MAX_CLIP || tx < 1 || tx > TSDRGPU_CLAHE_MAX_TILES ||
-		    ty < 1 || ty > TSDRGPU_CLAHE_MAX_TILES) return TSDRGPU_EINVAL;
-		p->ct_clip = clip_centi; p->ct_tx = tx; p->ct_ty = ty;
-	}
+	if (!p || !contrast_ok(mode, clip_centi, tx, ty)) return TSDRGPU_EINVAL;
+	if (mode == TSDRGPU_CONTRAST_CLAHE) { p->ct_clip = clip_centi; p->ct_tx = tx; p->ct_ty = ty; }
 	p->ct_mode = mode;
 	return TSDRGPU_OK;
 }
@@ -755,12 +752,8 @@ int tsdrgpu_pipeline_set_channel(tsdrgpu_pipeline_t *p, const tsdrgpu_channel_t 
 	return TSDRGPU_OK;
 }
 int tsdrgpu_pipeline_set_denoise(tsdrgpu_pipeline_t *p, int mode, int h_milli, int r, int p_radius) {
-	if (!p || (mode != TSDRGPU_DENOISE_OFF && mode != TSDRGPU_DENOISE_NLM)) return TSDRGPU_EINVAL;
-	if (mode == TSDRGPU_DENOISE_NLM) {
-		if (h_milli < 1 || h_milli > TSDRGPU_NLM_MAX_H || r < 1 || r > TSDRGPU_NLM_MAX_R || p_radius < 1 ||
-		    p_radius > TSDRGPU_NLM_MAX_P) return TSDRGPU_EINVAL;
-		p->nl_h = h_milli; p->nl_r = r; p->nl_p = p_radius;
-	}
+	if (!p || !denoise_ok(mode, h_milli, r, p_radius)) return TSDRGPU_EINVAL;
+	if (mode == TSDRGPU_DENOISE_NLM) { p->nl_h = h_milli; p->nl_r = r; p->nl_p = p_radius; }
 	p->nl_mode = mode;
 	return TSDRGPU_OK;
 }

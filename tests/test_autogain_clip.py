@@ -1,7 +1,9 @@
 """Percentile auto-gain (clip mode, include/tsdrgpu.h): the reference of tests/autogain_clip_model.py pinned to the oracle, then
 the GPU selection, frame stage, pipeline and host library against it."""
 import ctypes as C
+import math
 import os
+import re
 import threading
 import time
 
@@ -154,18 +156,28 @@ PERCENTS = ["0", "25", "25.0", "0.35", "1", "0.00005", "0.00015", "0.000049999",
             "25.00001", "30", "1e1", "0x1p2", " 1", "1 ", "1_0", "+1", "-0", "-1", ".5", "5.", "", "x", "1.2.3", "nan", "inf"]
 
 
+def _model_ppm(percent: str) -> int:
+    """tsdrgpu_autogain_ppm restated from tsdrgpu.h: digits with an optional fraction, value in [0, 25] -> floor(percent * 1e4 + 0.5);
+    else -1."""
+    if not re.fullmatch(r"[0-9]+(\.[0-9]+)?", percent):
+        return -1
+    v = float(percent)
+    return math.floor(v * 1e4 + 0.5) if v <= 25.0 else -1
+
+
 def test_autogain_spec_parsing():
-    """tsdrgpu_autogain_ppm (what the host library's TSDR_AUTOGAIN uses) and the Python parser agree on every spelling, including
-    halves of a ppm and 20 000 random decimals; only digits with an optional fraction, at most 25, are accepted."""
+    """tsdrgpu_autogain_ppm (what the host library's TSDR_AUTOGAIN and Python's auto-gain spelling use) agrees with the model on
+    every spelling, including halves of a ppm and 20 000 random decimals; only digits with an optional fraction, at most 25, are
+    accepted."""
     import random
     from tempestsdr_b200 import _native as N
     rng = random.Random(1)
     cases = PERCENTS + [f"{rng.randint(0, 25)}.{rng.randint(0, 10 ** rng.randint(1, 9))}" for _ in range(20_000)]
     lib = N.lib()
     for c in cases:
-        assert lib.tsdrgpu_autogain_ppm(c.encode()) == N.autogain_ppm(c), c
-    assert [N.autogain_ppm(c) for c in PERCENTS[:11]] == [0, 250_000, 250_000, 3500, 10_000, 1, 1, 0, 123_457, 249_999, 31_416]
-    assert all(N.autogain_ppm(c) == -1 for c in PERCENTS[11:])
+        assert lib.tsdrgpu_autogain_ppm(c.encode()) == _model_ppm(c), c
+    assert [_model_ppm(c) for c in PERCENTS[:11]] == [0, 250_000, 250_000, 3500, 10_000, 1, 1, 0, 123_457, 249_999, 31_416]
+    assert all(_model_ppm(c) == -1 for c in PERCENTS[11:])
     assert N.autogain_mode("minmax") == (N.AG_MINMAX, 0)
     assert N.autogain_mode("clip:0.35") == (N.AG_CLIP, 3500)
     for bad in ["clip:" + c for c in PERCENTS[11:]] + ["max", "clip"]:
