@@ -98,22 +98,27 @@ struct tsdrgpu_chanfilt {
 	tsdrgpu_ctx_t *ctx;
 	int T;                                    // 0: no spec set yet
 	float h_taps[2 * CF_TMAX];                // the taps of the current spec (host copy)
-	float2 *d_taps; int taps_dirty;           // device copy, uploaded by the next run when dirty
-	float2 *d_hist[2]; int hist_cur; int hist_zero;      // last T-1 pairs: runs read d_hist[hist_cur], write the other
+	DeviceBuf<float2> d_taps; int taps_dirty; // device copy, uploaded by the next run when dirty
+	DeviceBuf<float2> d_hist[2]; int hist_cur; int hist_zero;      // last T-1 pairs: runs read d_hist[hist_cur], write the other
 };
 
 extern "C" {
 
+static int create_handles(tsdrgpu_chanfilt *f) {
+	CU_TRY(f->ctx, f->d_taps.assign(CF_TMAX));
+	for (DeviceBuf<float2> &h : f->d_hist) {
+		CU_TRY(f->ctx, h.assign(CF_HMAX));
+		CU_TRY(f->ctx, cudaMemset(h.ptr, 0, sizeof(float2) * CF_HMAX));
+	}
+	return TSDRGPU_OK;
+}
+
 int tsdrgpu_chanfilt_create(tsdrgpu_ctx_t *ctx, tsdrgpu_chanfilt_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
-	tsdrgpu_chanfilt *f = new tsdrgpu_chanfilt();
-	memset(f, 0, sizeof(*f));
+	tsdrgpu_chanfilt *f = new tsdrgpu_chanfilt();      // value-initialised: every field not set here starts at zero
 	f->ctx = ctx;
-	CU_TRY(ctx, cudaMalloc(&f->d_taps, sizeof(float2) * CF_TMAX));
-	for (int i = 0; i < 2; i++) {
-		CU_TRY(ctx, cudaMalloc(&f->d_hist[i], sizeof(float2) * CF_HMAX));
-		CU_TRY(ctx, cudaMemset(f->d_hist[i], 0, sizeof(float2) * CF_HMAX));
-	}
+	const int rc = create_handles(f);
+	if (rc) { delete f; return rc; }                   // no stream or event of its own: its buffers go with it
 	*out = f;
 	return TSDRGPU_OK;
 }
@@ -122,14 +127,13 @@ void tsdrgpu_chanfilt_destroy(tsdrgpu_chanfilt_t *f) {
 	if (!f) return;
 	cudaSetDevice(f->ctx->device);
 	cudaDeviceSynchronize();
-	cudaFree(f->d_taps); cudaFree(f->d_hist[0]); cudaFree(f->d_hist[1]);
 	delete f;
 }
 
 int tsdrgpu_chanfilt_reset(tsdrgpu_chanfilt_t *f, void *stream) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, f != NULL);
 	BIND(f->ctx);
-	CU_TRY(f->ctx, cudaMemsetAsync(f->d_hist[f->hist_cur], 0, sizeof(float2) * CF_HMAX, (cudaStream_t) stream));
+	CU_TRY(f->ctx, cudaMemsetAsync(f->d_hist[f->hist_cur].ptr, 0, sizeof(float2) * CF_HMAX, (cudaStream_t) stream));
 	f->hist_zero = 0;
 	return TSDRGPU_OK;
 }
@@ -159,13 +163,13 @@ int tsdrgpu_chanfilt_run(tsdrgpu_chanfilt_t *f, void *stream_, const float *d_in
 	ARG_TRY(ctx, (a & 7u) == 0 && (b & 7u) == 0);
 	ARG_TRY(ctx, a + bytes <= b || b + bytes <= a);           // no overlap
 	if (f->taps_dirty) {                                      // pageable source: the copy is staged before the call returns
-		CU_TRY(ctx, cudaMemcpyAsync(f->d_taps, f->h_taps, sizeof(float) * 2 * f->T, cudaMemcpyHostToDevice, stream));
+		CU_TRY(ctx, cudaMemcpyAsync(f->d_taps.ptr, f->h_taps, sizeof(float) * 2 * f->T, cudaMemcpyHostToDevice, stream));
 		f->taps_dirty = 0;
 	}
-	if (f->hist_zero) { CU_TRY(ctx, cudaMemsetAsync(f->d_hist[f->hist_cur], 0, sizeof(float2) * CF_HMAX, stream)); f->hist_zero = 0; }
+	if (f->hist_zero) { CU_TRY(ctx, cudaMemsetAsync(f->d_hist[f->hist_cur].ptr, 0, sizeof(float2) * CF_HMAX, stream)); f->hist_zero = 0; }
 	const unsigned grid = (unsigned) ((pairs + CF_P - 1) / CF_P);
 	KL(ctx, "cf_fir", stream, cf_fir<<<grid, CF_THREADS, 0, stream>>>(reinterpret_cast<const float2 *>(d_in), reinterpret_cast<float2 *>(d_out), pairs,
-	                                                              f->d_taps, f->T, f->d_hist[f->hist_cur], f->d_hist[f->hist_cur ^ 1]));
+	                                                              f->d_taps.ptr, f->T, f->d_hist[f->hist_cur].ptr, f->d_hist[f->hist_cur ^ 1].ptr));
 	f->hist_cur ^= 1;
 	return TSDRGPU_OK;
 }

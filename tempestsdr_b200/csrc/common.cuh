@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/tsdrgpu.h"
+#include "devbuf.h"
 
 struct tsdrgpu_ctx {
 	int device;
@@ -15,10 +16,8 @@ struct tsdrgpu_ctx {
 	char err[512];
 	uint64_t launches;
 	// scratch owned by the context (grown on demand, reused across calls on the same stream)
-	void *scratch[4];
-	size_t scratch_bytes[4];
-	void *pinned;            // small pinned staging area for descriptor uploads / scalar read-backs
-	size_t pinned_bytes;
+	DeviceBuf<unsigned char> scratch[4];
+	PinnedBuf<unsigned char> pinned;      // small pinned staging area for descriptor uploads / scalar read-backs
 	std::mutex mu;
 	// optional per-kernel timing (bench.py's roofline): CUDA events on the launching stream around named launches
 	bool profiling;
@@ -112,9 +111,8 @@ int fs_copy_async(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, floa
 struct EnhanceState {
 	int contrast, clip_centi, tx, ty;            // TSDRGPU_CONTRAST_* and its parameters
 	int denoise, h_milli, r, p;                  // TSDRGPU_DENOISE_* and its parameters (R, P)
-	unsigned *d_clahe; size_t clahe_bytes;       // CLAHE histograms / LUTs of one pass
-	float *d_nlm; size_t nlm_bytes;              // NLM output of a batch
+	DeviceBuf<unsigned> d_clahe;                 // CLAHE histograms / LUTs of one pass
+	DeviceBuf<float> d_nlm;                      // NLM output of a batch
 };
 int enhance_reserve(tsdrgpu_ctx_t *ctx, EnhanceState *st, int nframes, int w, int h);
 int enhance_run(tsdrgpu_ctx_t *ctx, const EnhanceState *st, cudaStream_t stream, float *d_frames, int nframes, int w, int h);
-void enhance_free(EnhanceState *st);

@@ -40,8 +40,6 @@ int tsdrgpu_create(tsdrgpu_ctx_t **out, int device) {
 	c->sm_count = prop.multiProcessorCount;
 	c->err[0] = 0;
 	c->launches = 0;
-	for (int i = 0; i < 4; i++) { c->scratch[i] = NULL; c->scratch_bytes[i] = 0; }
-	c->pinned = NULL; c->pinned_bytes = 0;
 	c->profiling = false; c->prof_nnames = 0;
 	e = cudaSetDevice(device);
 	if (e != cudaSuccess) { delete c; return tsdrgpu_fail(NULL, TSDRGPU_ECUDA, "cudaSetDevice", e, __FILE__, __LINE__); }
@@ -52,8 +50,6 @@ int tsdrgpu_create(tsdrgpu_ctx_t **out, int device) {
 void tsdrgpu_destroy(tsdrgpu_ctx_t *ctx) {
 	if (!ctx) return;
 	cudaSetDevice(ctx->device);
-	for (int i = 0; i < 4; i++) if (ctx->scratch[i]) cudaFree(ctx->scratch[i]);
-	if (ctx->pinned) cudaFreeHost(ctx->pinned);
 	for (auto &r : ctx->prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
 	for (auto e : ctx->prof_pool) cudaEventDestroy(e);
 	delete ctx;
@@ -211,23 +207,22 @@ void tsdrgpu_prof_end(tsdrgpu_ctx_t *ctx, cudaStream_t stream) {
 }
 
 int tsdrgpu_scratch(tsdrgpu_ctx_t *ctx, int slot, size_t bytes, void **out) {
-	if (ctx->scratch_bytes[slot] < bytes) {
-		if (ctx->scratch[slot]) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, cudaFree(ctx->scratch[slot])); ctx->scratch[slot] = NULL; ctx->scratch_bytes[slot] = 0; }
-		size_t want = bytes + (bytes >> 2) + 256;
-		CU_TRY(ctx, cudaMalloc(&ctx->scratch[slot], want));
-		ctx->scratch_bytes[slot] = want;
+	DeviceBuf<unsigned char> &b = ctx->scratch[slot];
+	if (b.cap < bytes) {
+		if (b.ptr) CU_TRY(ctx, cudaDeviceSynchronize());
+		CU_TRY(ctx, b.assign(bytes + (bytes >> 2) + 256));
 	}
-	*out = ctx->scratch[slot];
+	*out = b.ptr;
 	return TSDRGPU_OK;
 }
 
 int tsdrgpu_pinned(tsdrgpu_ctx_t *ctx, size_t bytes, void **out) {
-	if (ctx->pinned_bytes < bytes) {
-		if (ctx->pinned) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, cudaFreeHost(ctx->pinned)); ctx->pinned = NULL; ctx->pinned_bytes = 0; }
-		size_t want = bytes * 2 + 4096;
-		{ int rc_ = tsdrgpu_malloc_host(ctx, want, &ctx->pinned); if (rc_) return rc_; }
-		ctx->pinned_bytes = want;
+	PinnedBuf<unsigned char> &b = ctx->pinned;
+	if (b.cap < bytes) {
+		if (b.ptr) CU_TRY(ctx, cudaDeviceSynchronize());
+		const int rc = b.assign(ctx, bytes * 2 + 4096);
+		if (rc) return rc;
 	}
-	*out = ctx->pinned;
+	*out = b.ptr;
 	return TSDRGPU_OK;
 }

@@ -360,18 +360,18 @@ static int fs_clahe_batch(tsdrgpu_ctx_t *ctx, const EnhanceState *st, cudaStream
 	CU_TRY(ctx, cudaFuncSetAttribute(fs_clahe_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) hist_smem));
 	for (int f0 = 0; f0 < nframes; f0 += g.fpp) {
 		const int nf = (nframes - f0 < g.fpp) ? nframes - f0 : g.fpp;
-		CU_TRY(ctx, cudaMemsetAsync(st->d_clahe, 0, sizeof(unsigned) * nf * g.tx * g.ty * CH_BINS, stream));
+		CU_TRY(ctx, cudaMemsetAsync(st->d_clahe.ptr, 0, sizeof(unsigned) * nf * g.tx * g.ty * CH_BINS, stream));
 		int parts = (target + nf * g.ty - 1) / (nf * g.ty);
 		if (parts > h / g.ty) parts = h / g.ty;          // every part keeps at least one row
 		if (parts < 1) parts = 1;
-		KL(ctx, "fs_clahe_hist", stream, fs_clahe_hist<<<dim3((unsigned) (g.ty * parts), nf), 256, hist_smem, stream>>>(in + f0 * n, w, h, g.tx, g.ty, parts, st->d_clahe));
-		KL(ctx, "fs_clahe_lut", stream, fs_clahe_lut<<<dim3((unsigned) (g.tx * g.ty), nf), CH_BINS, 0, stream>>>(st->d_clahe, st->clip_centi));
+		KL(ctx, "fs_clahe_hist", stream, fs_clahe_hist<<<dim3((unsigned) (g.ty * parts), nf), 256, hist_smem, stream>>>(in + f0 * n, w, h, g.tx, g.ty, parts, st->d_clahe.ptr));
+		KL(ctx, "fs_clahe_lut", stream, fs_clahe_lut<<<dim3((unsigned) (g.tx * g.ty), nf), CH_BINS, 0, stream>>>(st->d_clahe.ptr, st->clip_centi));
 		int bands = (2 * target + nf - 1) / nf;          // mapping CTAs: about eight per SM
 		if (bands > h) bands = h;
 		const int bh = (h + bands - 1) / bands;
 		bands = (h + bh - 1) / bh;
 		const size_t map_smem = sizeof(float) * ((size_t) stage_rows * g.tx * CH_BINS + w + bh) + sizeof(uchar2) * ((size_t) w + bh);
-		const float *luts = reinterpret_cast<const float *>(st->d_clahe);
+		const float *luts = reinterpret_cast<const float *>(st->d_clahe.ptr);
 		const auto map = vec ? fs_clahe_map<true> : fs_clahe_map<false>;
 		CU_TRY(ctx, cudaFuncSetAttribute(map, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) map_smem));
 		KL(ctx, "fs_clahe_map", stream, map<<<dim3((unsigned) bands, nf), 256, map_smem, stream>>>(in + f0 * n, out + f0 * n, w, h, g.tx, g.ty, bh, stage_rows, luts));
@@ -379,20 +379,14 @@ static int fs_clahe_batch(tsdrgpu_ctx_t *ctx, const EnhanceState *st, cudaStream
 	return TSDRGPU_OK;
 }
 
-// grows *buf to at least `bytes`; nothing may be in flight on it
-static int grow(tsdrgpu_ctx_t *ctx, void **buf, size_t *cap, size_t bytes) {
-	if (*cap >= bytes) return TSDRGPU_OK;
-	CU_TRY(ctx, cudaDeviceSynchronize());
-	if (*buf) CU_TRY(ctx, cudaFree(*buf));
-	CU_TRY(ctx, cudaMalloc(buf, bytes));
-	*cap = bytes;
-	return TSDRGPU_OK;
-}
-
+// the buffers the enabled steps need, each grown to exactly its size when short; nothing may be in flight on them
 int enhance_reserve(tsdrgpu_ctx_t *ctx, EnhanceState *st, int nframes, int w, int h) {
-	const int rc = st->denoise != TSDRGPU_DENOISE_NLM ? TSDRGPU_OK : grow(ctx, (void **) &st->d_nlm, &st->nlm_bytes, sizeof(float) * nframes * w * h);
-	if (rc || st->contrast != TSDRGPU_CONTRAST_CLAHE) return rc;
-	return grow(ctx, (void **) &st->d_clahe, &st->clahe_bytes, sizeof(unsigned) * ch_geom(st, nframes, w, h).words);
+	const size_t nlm = (size_t) nframes * w * h;
+	if (st->denoise == TSDRGPU_DENOISE_NLM && st->d_nlm.cap < nlm) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, st->d_nlm.assign(nlm)); }
+	if (st->contrast != TSDRGPU_CONTRAST_CLAHE) return TSDRGPU_OK;
+	const size_t words = ch_geom(st, nframes, w, h).words;
+	if (st->d_clahe.cap < words) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, st->d_clahe.assign(words)); }
+	return TSDRGPU_OK;
 }
 
 // NLM, then CLAHE, in place on nframes frames of w x h, on `stream`.  NLM cannot run in place: it writes the state's own scratch
@@ -401,13 +395,11 @@ int enhance_reserve(tsdrgpu_ctx_t *ctx, EnhanceState *st, int nframes, int w, in
 // with the next batch, so neither can be borrowed.
 int enhance_run(tsdrgpu_ctx_t *ctx, const EnhanceState *st, cudaStream_t stream, float *d_frames, int nframes, int w, int h) {
 	const bool nlm = st->denoise == TSDRGPU_DENOISE_NLM, clahe = st->contrast == TSDRGPU_CONTRAST_CLAHE;
-	const int rc = nlm ? fs_nlm_batch(ctx, stream, d_frames, st->d_nlm, nframes, w, h, st->h_milli, st->r, st->p) : TSDRGPU_OK;
+	const int rc = nlm ? fs_nlm_batch(ctx, stream, d_frames, st->d_nlm.ptr, nframes, w, h, st->h_milli, st->r, st->p) : TSDRGPU_OK;
 	if (rc || !(nlm || clahe)) return rc;
-	if (clahe) return fs_clahe_batch(ctx, st, stream, nlm ? st->d_nlm : d_frames, d_frames, nframes, w, h);
-	return fs_copy_async(ctx, stream, st->d_nlm, d_frames, (size_t) nframes * w * h);
+	if (clahe) return fs_clahe_batch(ctx, st, stream, nlm ? st->d_nlm.ptr : d_frames, d_frames, nframes, w, h);
+	return fs_copy_async(ctx, stream, st->d_nlm.ptr, d_frames, (size_t) nframes * w * h);
 }
-
-void enhance_free(EnhanceState *st) { cudaFree(st->d_clahe); cudaFree(st->d_nlm); }     // cudaFree(NULL) does nothing
 
 extern "C" {
 
@@ -422,9 +414,8 @@ int tsdrgpu_clahe(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_in, float *d
 	EnhanceState st = {TSDRGPU_CONTRAST_CLAHE, clip_centi, tx, ty};           // the rest zero: no denoise, no buffers yet
 	int rc = enhance_reserve(ctx, &st, nframes, w, h);
 	if (rc == TSDRGPU_OK) rc = fs_clahe_batch(ctx, &st, stream, d_in, d_out, nframes, w, h);
-	const cudaError_t e = cudaStreamSynchronize(stream);          // before the buffers go
+	const cudaError_t e = cudaStreamSynchronize(stream);          // before the buffers go with st
 	if (rc == TSDRGPU_OK && e != cudaSuccess) rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "tsdrgpu_clahe", e, __FILE__, __LINE__);
-	enhance_free(&st);
 	return rc;
 }
 

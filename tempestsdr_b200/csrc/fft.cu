@@ -870,16 +870,16 @@ int tsdrgpu_argmax_mag_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const f
 
 struct tsdrgpu_frd {
 	tsdrgpu_ctx_t *ctx;
-	float *d_big; size_t big_cap;                 // extbuff (2*size floats), only where the answers are materialised (see frd_run_impl)
-	double *d_p1, *d_p2; size_t p1_cap, p2_cap;   // the two running means
+	DeviceBuf<float> d_big;                       // extbuff (2*size floats), only where the answers are materialised (see frd_run_impl)
+	DeviceBuf<double> d_p1, d_p2;                 // the two running means, one element more than the plots
 	uint64_t calls; int fresh;
-	int *d_peaks;                                 // first strict maximum of each plot (k_plot_peaks), refreshed with every run
+	DeviceBuf<int> d_peaks;                       // first strict maximum of each plot (k_plot_peaks), refreshed with every run
 	// overlapped mode (tsdrgpu_frd_set_overlap): everything a run launches goes to an internal stream, behind what the caller's
 	// stream held at the call, with work buffers of its own -- the transforms then share the chip with whatever the caller
 	// enqueues next (the pass kernels are bound by issue slots, the resampler and the frame stage by other things)
 	int overlap, pending;
 	cudaStream_t s_side; cudaEvent_t ev_in, ev_done;
-	float2 *w0, *w1; size_t w0_cap, w1_cap;
+	DeviceBuf<float2> w0, w1;
 };
 
 extern "C" {
@@ -1051,14 +1051,46 @@ int tsdrgpu_accumulate(tsdrgpu_ctx_t *ctx, void *stream, double *d_out, uint64_t
 }
 
 // ---- frame-rate detector ---------------------------------------------------------------------------------------
+// the side stream and its two events, whichever exist
+static void destroy_side(tsdrgpu_frd *f) {
+	if (f->s_side) cudaStreamDestroy(f->s_side);
+	if (f->ev_in) cudaEventDestroy(f->ev_in);
+	if (f->ev_done) cudaEventDestroy(f->ev_done);
+	f->s_side = NULL; f->ev_in = f->ev_done = NULL;
+}
+// a detector whole or half built; its buffers go with the object
+static void release(tsdrgpu_frd *f) {
+	destroy_side(f);
+	delete f;
+}
+
+static int create_handles(tsdrgpu_frd *f) {
+	CU_TRY(f->ctx, f->d_peaks.assign(64));
+	CU_TRY(f->ctx, cudaMemset(f->d_peaks.ptr, 0, 256));
+	return TSDRGPU_OK;
+}
+
 int tsdrgpu_frd_create(tsdrgpu_ctx_t *ctx, tsdrgpu_frd_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
-	tsdrgpu_frd *f = new tsdrgpu_frd();
-	memset(f, 0, sizeof *f);
+	tsdrgpu_frd *f = new tsdrgpu_frd();      // value-initialised: every field not set here starts at zero
 	f->ctx = ctx; f->fresh = 1;
-	CU_TRY(ctx, cudaMalloc(&f->d_peaks, 256));
-	CU_TRY(ctx, cudaMemset(f->d_peaks, 0, 256));
+	const int rc = create_handles(f);
+	if (rc) { release(f); return rc; }
 	*out = f;
+	return TSDRGPU_OK;
+}
+// the side stream and its two events, all three or none
+static int create_side(tsdrgpu_frd *f) {
+	tsdrgpu_ctx_t *ctx = f->ctx;
+	// the detector's work is background work (a plot every few frames): lowest priority, so that the block scheduler hands free
+	// SM resources to the pixel path first and lets the transforms fill what is left (TSDRGPU_FRD_PRIO=high|default for studies)
+	int lo = 0, hi = 0;
+	CU_TRY(ctx, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+	const char *pr = getenv("TSDRGPU_FRD_PRIO");
+	const int prio = (pr && !strcmp(pr, "high")) ? hi : ((pr && !strcmp(pr, "default")) ? 0 : lo);
+	CU_TRY(ctx, cudaStreamCreateWithPriority(&f->s_side, cudaStreamNonBlocking, prio));
+	CU_TRY(ctx, cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
+	CU_TRY(ctx, cudaEventCreateWithFlags(&f->ev_done, cudaEventDisableTiming));
 	return TSDRGPU_OK;
 }
 // overlapped mode on/off (see struct tsdrgpu_frd).  While it is on, a capture handed to tsdrgpu_frd_run* must stay untouched
@@ -1068,15 +1100,8 @@ int tsdrgpu_frd_set_overlap(tsdrgpu_frd_t *f, int on) {
 	tsdrgpu_ctx_t *ctx = f->ctx;
 	BIND(ctx);
 	if (on && !f->s_side) {
-		// the detector's work is background work (a plot every few frames): lowest priority, so that the block scheduler hands free
-		// SM resources to the pixel path first and lets the transforms fill what is left (TSDRGPU_FRD_PRIO=high|default for studies)
-		int lo = 0, hi = 0;
-		CU_TRY(ctx, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-		const char *pr = getenv("TSDRGPU_FRD_PRIO");
-		const int prio = (pr && !strcmp(pr, "high")) ? hi : ((pr && !strcmp(pr, "default")) ? 0 : lo);
-		CU_TRY(ctx, cudaStreamCreateWithPriority(&f->s_side, cudaStreamNonBlocking, prio));
-		CU_TRY(ctx, cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
-		CU_TRY(ctx, cudaEventCreateWithFlags(&f->ev_done, cudaEventDisableTiming));
+		const int rc = create_side(f);
+		if (rc) { destroy_side(f); return rc; }         // none of the three stays: the next call starts again
 	}
 	if (!on && f->pending) { CU_TRY(ctx, cudaStreamSynchronize(f->s_side)); f->pending = 0; }
 	f->overlap = on ? 1 : 0;
@@ -1092,14 +1117,7 @@ int tsdrgpu_frd_join(tsdrgpu_frd_t *f, void *stream) {
 void tsdrgpu_frd_destroy(tsdrgpu_frd_t *f) {
 	if (!f) return;
 	cudaSetDevice(f->ctx->device); cudaDeviceSynchronize();
-	if (f->d_big) cudaFree(f->d_big);
-	if (f->d_p1) cudaFree(f->d_p1);
-	if (f->d_p2) cudaFree(f->d_p2);
-	if (f->d_peaks) cudaFree(f->d_peaks);
-	if (f->w0) cudaFree(f->w0);
-	if (f->w1) cudaFree(f->w1);
-	if (f->s_side) { cudaStreamDestroy(f->s_side); cudaEventDestroy(f->ev_in); cudaEventDestroy(f->ev_done); }
-	delete f;
+	release(f);
 }
 int tsdrgpu_frd_reset(tsdrgpu_frd_t *f) { if (!f) return TSDRGPU_EINVAL; f->fresh = 1; return TSDRGPU_OK; }
 
@@ -1132,25 +1150,22 @@ static int frd_run_impl(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, co
 		// the internal stream picks up behind everything the caller's stream holds now (the capture is complete there)
 		stream = f->s_side;
 		const size_t need0 = (size_t) N * batch, need1 = (size_t) (N / 2) * batch + 16;
-		if (f->w0_cap < need0 || f->w1_cap < need1) {
+		if (f->w0.cap < need0 || f->w1.cap < need1) {
 			CU_TRY(ctx, cudaStreamSynchronize(f->s_side));
-			if (f->w0) CU_TRY(ctx, cudaFree(f->w0));
-			if (f->w1) CU_TRY(ctx, cudaFree(f->w1));
-			f->w0 = f->w1 = NULL; f->w0_cap = f->w1_cap = 0;
-			CU_TRY(ctx, cudaMalloc(&f->w0, sizeof(float2) * need0)); f->w0_cap = need0;
-			CU_TRY(ctx, cudaMalloc(&f->w1, sizeof(float2) * need1)); f->w1_cap = need1;
+			CU_TRY(ctx, f->w0.assign(need0));
+			CU_TRY(ctx, f->w1.assign(need1));
 		}
-		wb = WorkBufs{f->w0, f->w1};
+		wb = WorkBufs{f->w0.ptr, f->w1.ptr};
 		CU_TRY(ctx, cudaEventRecord(f->ev_in, caller));
 		CU_TRY(ctx, cudaStreamWaitEvent(f->s_side, f->ev_in, 0));
 	}
-	if (f->p1_cap < (size_t) flen || f->fresh) {
-		if (f->p1_cap < (size_t) flen) { CU_TRY(ctx, cudaStreamSynchronize(stream)); if (f->d_p1) CU_TRY(ctx, cudaFree(f->d_p1)); CU_TRY(ctx, cudaMalloc(&f->d_p1, sizeof(double) * (flen + 1))); f->p1_cap = flen; }
-		CU_TRY(ctx, cudaMemsetAsync(f->d_p1, 0, sizeof(double) * (flen + 1), stream));
+	if (f->d_p1.cap <= (size_t) flen || f->fresh) {
+		if (f->d_p1.cap <= (size_t) flen) { CU_TRY(ctx, cudaStreamSynchronize(stream)); CU_TRY(ctx, f->d_p1.assign((size_t) flen + 1)); }
+		CU_TRY(ctx, cudaMemsetAsync(f->d_p1.ptr, 0, sizeof(double) * (flen + 1), stream));
 	}
-	if (f->p2_cap < (size_t) llen || f->fresh) {
-		if (f->p2_cap < (size_t) llen) { CU_TRY(ctx, cudaStreamSynchronize(stream)); if (f->d_p2) CU_TRY(ctx, cudaFree(f->d_p2)); CU_TRY(ctx, cudaMalloc(&f->d_p2, sizeof(double) * (llen + 1))); f->p2_cap = llen; }
-		CU_TRY(ctx, cudaMemsetAsync(f->d_p2, 0, sizeof(double) * (llen + 1), stream));
+	if (f->d_p2.cap <= (size_t) llen || f->fresh) {
+		if (f->d_p2.cap <= (size_t) llen) { CU_TRY(ctx, cudaStreamSynchronize(stream)); CU_TRY(ctx, f->d_p2.assign((size_t) llen + 1)); }
+		CU_TRY(ctx, cudaMemsetAsync(f->d_p2.ptr, 0, sizeof(double) * (llen + 1), stream));
 	}
 	if (f->fresh) { f->calls = 0; f->fresh = 0; }
 	const uint64_t first_calls = f->calls + 1;                  // extbuffer.c:81, one prepare per capture
@@ -1159,24 +1174,23 @@ static int frd_run_impl(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, co
 	if (fold) {
 		// only the two lag windows are ever read (frameratedetector.c:106-109)
 		if ((rc = ensure_table(ctx, stream))) return rc;
-		const RunningMeans rm = {f->d_p1, f->d_p2, fmin, flen, lmin, llen, first_calls};
+		const RunningMeans rm = {f->d_p1.ptr, f->d_p2.ptr, fmin, flen, lmin, llen, first_calls};
 		if ((rc = autocorrelation_batch_half(ctx, stream, NULL, 0, d_capture, (long long) capture_stride, N, batch, &rm, wb))) return rc;
 	} else {
 		const size_t big_need = 2ull * size * batch;
-		if (f->big_cap < big_need) {
+		if (f->d_big.cap < big_need) {
 			CU_TRY(ctx, cudaStreamSynchronize(stream));
-			if (f->d_big) CU_TRY(ctx, cudaFree(f->d_big));
-			CU_TRY(ctx, cudaMalloc(&f->d_big, sizeof(float) * big_need)); f->big_cap = big_need;
+			CU_TRY(ctx, f->d_big.assign(big_need));
 		}
-		if ((rc = autocorrelation_batch(ctx, stream, f->d_big, 2ll * size, d_capture, (long long) capture_stride, size, batch, skip_tail, wb))) return rc;
-		if (flen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) flen, ctx->sm_count), 256, 0, stream>>>(f->d_p1, first_calls, reinterpret_cast<const float2 *>(f->d_big), (long long) size, batch, fmin, flen));
-		if (llen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) llen, ctx->sm_count), 256, 0, stream>>>(f->d_p2, first_calls, reinterpret_cast<const float2 *>(f->d_big), (long long) size, batch, lmin, llen));
+		if ((rc = autocorrelation_batch(ctx, stream, f->d_big.ptr, 2ll * size, d_capture, (long long) capture_stride, size, batch, skip_tail, wb))) return rc;
+		if (flen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) flen, ctx->sm_count), 256, 0, stream>>>(f->d_p1.ptr, first_calls, reinterpret_cast<const float2 *>(f->d_big.ptr), (long long) size, batch, fmin, flen));
+		if (llen) KL(ctx, "k_accumulate", stream, k_accumulate_batch<<<grid1d((unsigned long long) llen, ctx->sm_count), 256, 0, stream>>>(f->d_p2.ptr, first_calls, reinterpret_cast<const float2 *>(f->d_big.ptr), (long long) size, batch, lmin, llen));
 	}
-	KL(ctx, "k_plot_peaks", stream, k_plot_peaks<<<2, 1024, 0, stream>>>(f->d_p1, flen, f->d_p2, llen, f->d_peaks));
+	KL(ctx, "k_plot_peaks", stream, k_plot_peaks<<<2, 1024, 0, stream>>>(f->d_p1.ptr, flen, f->d_p2.ptr, llen, f->d_peaks.ptr));
 	if (calls) *calls = f->calls;
 	if (h_frame_plot || h_line_plot) {
-		if (h_frame_plot) CU_TRY(ctx, cudaMemcpyAsync(h_frame_plot, f->d_p1, sizeof(double) * (size_t) (flen < frame_cap ? flen : frame_cap), cudaMemcpyDeviceToHost, stream));
-		if (h_line_plot) CU_TRY(ctx, cudaMemcpyAsync(h_line_plot, f->d_p2, sizeof(double) * (size_t) (llen < line_cap ? llen : line_cap), cudaMemcpyDeviceToHost, stream));
+		if (h_frame_plot) CU_TRY(ctx, cudaMemcpyAsync(h_frame_plot, f->d_p1.ptr, sizeof(double) * (size_t) (flen < frame_cap ? flen : frame_cap), cudaMemcpyDeviceToHost, stream));
+		if (h_line_plot) CU_TRY(ctx, cudaMemcpyAsync(h_line_plot, f->d_p2.ptr, sizeof(double) * (size_t) (llen < line_cap ? llen : line_cap), cudaMemcpyDeviceToHost, stream));
 		if (synchronise) CU_TRY(ctx, cudaStreamSynchronize(stream));
 	}
 	if (f->overlap) { CU_TRY(ctx, cudaEventRecord(f->ev_done, f->s_side)); f->pending = 1; }
@@ -1206,17 +1220,18 @@ int tsdrgpu_frd_dump_csv(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, c
 	BIND(ctx); ARG_TRY(ctx, d_capture != NULL && size > 0 && path != NULL && samplerate > 0);
 	cudaStream_t stream = (cudaStream_t) stream_;
 	const uint32_t maxels = tsdrgpu_fft_getrealsize(2u * size) / 2u;           // floats of the answer the reference walks
-	float *d_ans = NULL;
-	CU_TRY(ctx, cudaMalloc(&d_ans, sizeof(float) * 2ull * size));
-	int rc = autocorrelation_batch(ctx, stream, d_ans, 2ll * size, d_capture, (long long) size, size, 1, false);
 	std::vector<float> h(maxels);
-	if (rc == TSDRGPU_OK) {
-		const cudaError_t e1 = cudaMemcpyAsync(h.data(), d_ans, sizeof(float) * maxels, cudaMemcpyDeviceToHost, stream);
-		const cudaError_t e2 = (e1 == cudaSuccess) ? cudaStreamSynchronize(stream) : e1;
-		if (e2 != cudaSuccess) rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "autocorrelation dump: copy", e2, __FILE__, __LINE__);
-	} else cudaStreamSynchronize(stream);
-	cudaFree(d_ans);
-	if (rc != TSDRGPU_OK) return rc;
+	{   // the device answer goes at the end of this block, after the stream is done with it
+		DeviceBuf<float> d_ans;
+		CU_TRY(ctx, d_ans.assign(2ull * size));
+		int rc = autocorrelation_batch(ctx, stream, d_ans.ptr, 2ll * size, d_capture, (long long) size, size, 1, false);
+		if (rc == TSDRGPU_OK) {
+			const cudaError_t e1 = cudaMemcpyAsync(h.data(), d_ans.ptr, sizeof(float) * maxels, cudaMemcpyDeviceToHost, stream);
+			const cudaError_t e2 = (e1 == cudaSuccess) ? cudaStreamSynchronize(stream) : e1;
+			if (e2 != cudaSuccess) rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "autocorrelation dump: copy", e2, __FILE__, __LINE__);
+		} else cudaStreamSynchronize(stream);
+		if (rc != TSDRGPU_OK) return rc;
+	}
 	FILE *fp = fopen(path, "w");
 	if (!fp) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "autocorrelation dump: cannot open the file", cudaSuccess, __FILE__, __LINE__);
 	fprintf(fp, "%s, %s\n", "ms", "dB");
@@ -1239,10 +1254,10 @@ int tsdrgpu_frd_get_plots(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, 
 	int fmin, fmax, lmin, lmax;
 	tsdrgpu_frd_windows(samplerate, &fmin, &fmax, &lmin, &lmax);
 	const int flen = fmax - fmin, llen = lmax - lmin;
-	ARG_TRY(ctx, f->p1_cap >= (size_t) flen && f->p2_cap >= (size_t) llen);
+	ARG_TRY(ctx, f->d_p1.cap > (size_t) flen && f->d_p2.cap > (size_t) llen);
 	if (f->pending) CU_TRY(ctx, cudaStreamWaitEvent(stream, f->ev_done, 0));
-	if (h_frame_plot) CU_TRY(ctx, cudaMemcpyAsync(h_frame_plot, f->d_p1, sizeof(double) * (size_t) (flen < frame_cap ? flen : frame_cap), cudaMemcpyDeviceToHost, stream));
-	if (h_line_plot) CU_TRY(ctx, cudaMemcpyAsync(h_line_plot, f->d_p2, sizeof(double) * (size_t) (llen < line_cap ? llen : line_cap), cudaMemcpyDeviceToHost, stream));
+	if (h_frame_plot) CU_TRY(ctx, cudaMemcpyAsync(h_frame_plot, f->d_p1.ptr, sizeof(double) * (size_t) (flen < frame_cap ? flen : frame_cap), cudaMemcpyDeviceToHost, stream));
+	if (h_line_plot) CU_TRY(ctx, cudaMemcpyAsync(h_line_plot, f->d_p2.ptr, sizeof(double) * (size_t) (llen < line_cap ? llen : line_cap), cudaMemcpyDeviceToHost, stream));
 	CU_TRY(ctx, cudaStreamSynchronize(stream));
 	return TSDRGPU_OK;
 }
@@ -1266,14 +1281,14 @@ int tsdrgpu_frd_peaks_async(tsdrgpu_frd_t *f, void *stream, int32_t *h_peaks_pin
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, f != NULL && h_peaks_pinned != NULL);
 	BIND(f->ctx);
 	if (f->pending) CU_TRY(f->ctx, cudaStreamWaitEvent((cudaStream_t) stream, f->ev_done, 0));
-	CU_TRY(f->ctx, cudaMemcpyAsync(h_peaks_pinned, f->d_peaks, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t) stream));
+	CU_TRY(f->ctx, cudaMemcpyAsync(h_peaks_pinned, f->d_peaks.ptr, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t) stream));
 	return TSDRGPU_OK;
 }
 int tsdrgpu_frd_peaks(tsdrgpu_frd_t *f, void *stream, int32_t *h_peaks) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, f != NULL && h_peaks != NULL);
 	BIND(f->ctx);
 	if (f->pending) CU_TRY(f->ctx, cudaStreamWaitEvent((cudaStream_t) stream, f->ev_done, 0));
-	CU_TRY(f->ctx, cudaMemcpyAsync(h_peaks, f->d_peaks, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t) stream));
+	CU_TRY(f->ctx, cudaMemcpyAsync(h_peaks, f->d_peaks.ptr, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t) stream));
 	CU_TRY(f->ctx, cudaStreamSynchronize((cudaStream_t) stream));
 	return TSDRGPU_OK;
 }

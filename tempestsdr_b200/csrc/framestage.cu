@@ -1340,73 +1340,72 @@ int fs_copy_async(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, floa
 // -----------------------------------------------------------------------------------------------------------------
 struct tsdrgpu_framestage {
 	tsdrgpu_ctx_t *ctx;
-	float *d_screen; size_t screen_cap;          // dsp_postprocess_t.screenbuffer / bufsize
+	DeviceBuf<float> d_screen;                   // dsp_postprocess_t.screenbuffer / bufsize
 	int w, h; size_t n;                          // current geometry (pp->width/height/sizetopoll)
 	int lp_before_sync;                          // pp->lowpass_before_sync
 	int runs;                                    // pp->runs
-	SyncState *d_state;
+	DeviceBuf<SyncState> d_state;
 	// batch temporaries.  The sync search + re-centre of batch k may run on the side stream while the main stream
 	// already produces batch k+1, so everything they read is double-buffered ("phase" = batch parity).
-	float *d_t1, *d_t2[2]; size_t t_cap;
-	float *d_wstrips[2], *d_hstrips[2]; size_t strips_cap;
-	float *d_pmin, *d_pmax; double *d_psum, *d_psq, *d_plin; FrameParams *d_params; int batch_cap;
+	DeviceBuf<float> d_t1, d_t2[2];
+	DeviceBuf<float> d_wstrips[2], d_hstrips[2];
+	DeviceBuf<float> d_pmin, d_pmax; DeviceBuf<double> d_psum, d_psq, d_plin; DeviceBuf<FrameParams> d_params;
+	int batch_cap;                               // frames every per-batch buffer holds (0 until all of them are allocated)
 	int ag_mode, ag_ppm;                         // tsdrgpu_framestage_set_autogain (kept across reset)
-	unsigned *d_sel_hist; SelState *d_sel; float2 *d_levels;     // clip-mode selection, batch_cap frames
+	DeviceBuf<unsigned> d_sel_hist; DeviceBuf<SelState> d_sel; DeviceBuf<float2> d_levels;     // clip-mode selection, batch_cap frames
 	EnhanceState enh;                            // tsdrgpu_framestage_set_contrast / _set_denoise (kept across reset)
-	tsdrgpu_frame_result_t *d_results[2];
-	double *d_chain;
-	int *d_resume;                               // first frame of the batch fs_sync_walk could not serve from the tables
+	DeviceBuf<tsdrgpu_frame_result_t> d_results[2];
+	DeviceBuf<double> d_chain;
+	DeviceBuf<int> d_resume;                     // first frame of the batch fs_sync_walk could not serve from the tables
 	float taps[5];
 	int overlap, phase, side_pending;
-	double *d_prep; size_t prep_cap;             // fs_sync_prep's per-frame records (consumed by fs_sync on the same stream)
+	DeviceBuf<double> d_prep;                    // fs_sync_prep's per-frame records (consumed by fs_sync on the same stream)
 	cudaStream_t s_side;
 	cudaEvent_t ev_ready[2];                     // main: collapse of this phase done -> side may start
 	cudaEvent_t ev_done[2];                      // side: sync + emit of this phase done -> buffers of the phase are free
 	CollapseMaps collapse_maps[4];               // fs_collapse_tiles' tensor maps of the buffers collapsed last (d_t2[0/1], d_t1)
 };
 
+// hands a's buffer to b and b's to a (DeviceBuf can be neither copied nor moved)
+static void fs_exchange(DeviceBuf<float> &a, DeviceBuf<float> &b) { std::swap(a.ptr, b.ptr); std::swap(a.cap, b.cap); }
+
+// every buffer of a group at exactly n elements, all of them reallocated when one is short (a failed reallocation leaves that one
+// empty, so the next call tries again); the side stream may still be reading them
+template <class T, size_t K> static int fs_assign_group(tsdrgpu_ctx_t *ctx, DeviceBuf<T> *const (&bufs)[K], size_t n) {
+	bool grow = false;
+	for (DeviceBuf<T> *b : bufs) grow |= b->cap < n;
+	if (!grow) return TSDRGPU_OK;
+	CU_TRY(ctx, cudaDeviceSynchronize());
+	for (DeviceBuf<T> *b : bufs) CU_TRY(ctx, b->assign(n));
+	return TSDRGPU_OK;
+}
+
 static int fs_reserve(tsdrgpu_framestage *fs, int nframes, size_t n, int w, int h) {
 	tsdrgpu_ctx_t *ctx = fs->ctx;
-	const size_t need = (size_t) nframes * n;
-	if (fs->t_cap < need) {
-		CU_TRY(ctx, cudaDeviceSynchronize());
-		float **bufs[] = {&fs->d_t1, &fs->d_t2[0], &fs->d_t2[1]};
-		for (float **b : bufs) { if (*b) CU_TRY(ctx, cudaFree(*b)); CU_TRY(ctx, cudaMalloc(b, sizeof(float) * need)); }
-		fs->t_cap = need;
-	}
-	const size_t sneed = (size_t) nframes * (size_t) (w > h ? w : h);
-	if (fs->strips_cap < sneed) {
-		CU_TRY(ctx, cudaDeviceSynchronize());
-		float **bufs[] = {&fs->d_wstrips[0], &fs->d_wstrips[1], &fs->d_hstrips[0], &fs->d_hstrips[1]};
-		for (float **b : bufs) { if (*b) CU_TRY(ctx, cudaFree(*b)); CU_TRY(ctx, cudaMalloc(b, sizeof(float) * sneed)); }
-		fs->strips_cap = sneed;
-	}
-	const size_t pneed = (size_t) nframes * fs_prep_stride(w, h);
-	if (fs->prep_cap < pneed) {
-		CU_TRY(ctx, cudaDeviceSynchronize());
-		if (fs->d_prep) CU_TRY(ctx, cudaFree(fs->d_prep));
-		CU_TRY(ctx, cudaMalloc(&fs->d_prep, sizeof(double) * pneed));
-		fs->prep_cap = pneed;
-	}
+	int rc;
+	DeviceBuf<float> *const frames[] = {&fs->d_t1, &fs->d_t2[0], &fs->d_t2[1]};
+	if ((rc = fs_assign_group(ctx, frames, (size_t) nframes * n))) return rc;
+	DeviceBuf<float> *const strips[] = {&fs->d_wstrips[0], &fs->d_wstrips[1], &fs->d_hstrips[0], &fs->d_hstrips[1]};
+	if ((rc = fs_assign_group(ctx, strips, (size_t) nframes * (size_t) (w > h ? w : h)))) return rc;
+	DeviceBuf<double> *const prep[] = {&fs->d_prep};
+	if ((rc = fs_assign_group(ctx, prep, (size_t) nframes * fs_prep_stride(w, h)))) return rc;
 	if (fs->batch_cap < nframes) {
 		CU_TRY(ctx, cudaDeviceSynchronize());
-		void *ptrs[] = {fs->d_pmin, fs->d_pmax, fs->d_psum, fs->d_psq, fs->d_plin, fs->d_params, fs->d_results[0], fs->d_results[1],
-		                fs->d_sel_hist, fs->d_sel, fs->d_levels};
-		for (void *p : ptrs) if (p) CU_TRY(ctx, cudaFree(p));
+		fs->batch_cap = 0;
 		const size_t pc = (size_t) nframes * FS_MM_CHUNKS;
-		CU_TRY(ctx, cudaMalloc(&fs->d_pmin, sizeof(float) * pc));
-		CU_TRY(ctx, cudaMalloc(&fs->d_pmax, sizeof(float) * pc));
-		CU_TRY(ctx, cudaMalloc(&fs->d_psum, sizeof(double) * pc));
-		CU_TRY(ctx, cudaMalloc(&fs->d_psq, sizeof(double) * pc));
-		CU_TRY(ctx, cudaMalloc(&fs->d_plin, sizeof(double) * pc));
-		CU_TRY(ctx, cudaMalloc(&fs->d_params, sizeof(FrameParams) * nframes));
-		CU_TRY(ctx, cudaMalloc(&fs->d_sel_hist, sizeof(unsigned) * 2 * SEL_BINS * nframes));
-		CU_TRY(ctx, cudaMemset(fs->d_sel_hist, 0, sizeof(unsigned) * 2 * SEL_BINS * nframes));     // each scan re-zeroes what it read
-		CU_TRY(ctx, cudaMalloc(&fs->d_sel, sizeof(SelState) * nframes));
-		CU_TRY(ctx, cudaMalloc(&fs->d_levels, sizeof(float2) * nframes));
+		CU_TRY(ctx, fs->d_pmin.assign(pc));
+		CU_TRY(ctx, fs->d_pmax.assign(pc));
+		CU_TRY(ctx, fs->d_psum.assign(pc));
+		CU_TRY(ctx, fs->d_psq.assign(pc));
+		CU_TRY(ctx, fs->d_plin.assign(pc));
+		CU_TRY(ctx, fs->d_params.assign(nframes));
+		CU_TRY(ctx, fs->d_sel_hist.assign((size_t) 2 * SEL_BINS * nframes));
+		CU_TRY(ctx, cudaMemset(fs->d_sel_hist.ptr, 0, sizeof(unsigned) * 2 * SEL_BINS * nframes));     // each scan re-zeroes what it read
+		CU_TRY(ctx, fs->d_sel.assign(nframes));
+		CU_TRY(ctx, fs->d_levels.assign(nframes));
 		for (int i = 0; i < 2; i++) {
-			CU_TRY(ctx, cudaMalloc(&fs->d_results[i], sizeof(tsdrgpu_frame_result_t) * nframes));
-			CU_TRY(ctx, cudaMemset(fs->d_results[i], 0, sizeof(tsdrgpu_frame_result_t) * nframes));
+			CU_TRY(ctx, fs->d_results[i].assign(nframes));
+			CU_TRY(ctx, cudaMemset(fs->d_results[i].ptr, 0, sizeof(tsdrgpu_frame_result_t) * nframes));
 		}
 		// the memsets run on the legacy default stream, which does not order work on non-blocking streams (the pipeline's):
 		// the selection's first histogram round must see the zeroed counts
@@ -1421,13 +1420,13 @@ static int fs_select_batch(tsdrgpu_framestage *fs, cudaStream_t stream, const fl
                            bool snr) {
 	tsdrgpu_ctx_t *ctx = fs->ctx;
 	const dim3 grid(chunks, nframes);
-	if (snr) KL(ctx, "fs_select_hist", stream, (fs_select_hist<1, true><<<grid, 256, 0, stream>>>(in, n, fs->d_sel, fs->d_sel_hist, fs->d_psum)));
-	else KL(ctx, "fs_select_hist", stream, (fs_select_hist<1, false><<<grid, 256, 0, stream>>>(in, n, fs->d_sel, fs->d_sel_hist, fs->d_psum)));
-	KL(ctx, "fs_select_scan", stream, fs_select_scan<1><<<nframes, 256, 0, stream>>>(in, n, ppm, fs->d_sel, fs->d_sel_hist, fs->d_levels));
-	KL(ctx, "fs_select_hist", stream, (fs_select_hist<2, false><<<grid, 256, 0, stream>>>(in, n, fs->d_sel, fs->d_sel_hist, fs->d_psum)));
-	KL(ctx, "fs_select_scan", stream, fs_select_scan<2><<<nframes, 256, 0, stream>>>(in, n, ppm, fs->d_sel, fs->d_sel_hist, fs->d_levels));
-	KL(ctx, "fs_select_hist", stream, (fs_select_hist<3, false><<<grid, 256, 0, stream>>>(in, n, fs->d_sel, fs->d_sel_hist, fs->d_psum)));
-	KL(ctx, "fs_select_scan", stream, fs_select_scan<3><<<nframes, 256, 0, stream>>>(in, n, ppm, fs->d_sel, fs->d_sel_hist, fs->d_levels));
+	if (snr) KL(ctx, "fs_select_hist", stream, (fs_select_hist<1, true><<<grid, 256, 0, stream>>>(in, n, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_psum.ptr)));
+	else KL(ctx, "fs_select_hist", stream, (fs_select_hist<1, false><<<grid, 256, 0, stream>>>(in, n, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_psum.ptr)));
+	KL(ctx, "fs_select_scan", stream, fs_select_scan<1><<<nframes, 256, 0, stream>>>(in, n, ppm, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_levels.ptr));
+	KL(ctx, "fs_select_hist", stream, (fs_select_hist<2, false><<<grid, 256, 0, stream>>>(in, n, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_psum.ptr)));
+	KL(ctx, "fs_select_scan", stream, fs_select_scan<2><<<nframes, 256, 0, stream>>>(in, n, ppm, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_levels.ptr));
+	KL(ctx, "fs_select_hist", stream, (fs_select_hist<3, false><<<grid, 256, 0, stream>>>(in, n, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_psum.ptr)));
+	KL(ctx, "fs_select_scan", stream, fs_select_scan<3><<<nframes, 256, 0, stream>>>(in, n, ppm, fs->d_sel.ptr, fs->d_sel_hist.ptr, fs->d_levels.ptr));
 	return TSDRGPU_OK;
 }
 
@@ -1442,31 +1441,34 @@ static int fs_autogain_batch(tsdrgpu_framestage *fs, cudaStream_t stream, const 
 	const bool clip = fs->ag_mode == TSDRGPU_AG_CLIP;
 	int rc;
 	if (clip) { if ((rc = fs_select_batch(fs, stream, in, nframes, n, fs->ag_ppm, chunks, snr))) return rc; }
-	else if (snr) KL(ctx, "fs_minmax", stream, fs_minmax<true><<<grid, 256, 0, stream>>>(in, n, fs->d_pmin, fs->d_pmax, fs->d_psum));
-	else KL(ctx, "fs_minmax", stream, fs_minmax<false><<<grid, 256, 0, stream>>>(in, n, fs->d_pmin, fs->d_pmax, fs->d_psum));
-	KL(ctx, "fs_autogain_iir", stream, fs_autogain_iir<<<1, 256, 0, stream>>>(in, n, nframes, chunks, fs->d_pmin, fs->d_pmax, fs->d_psum, snr, norm, fs->d_state, fs->d_params,
-	                                                                         clip ? fs->d_levels : NULL));
+	else if (snr) KL(ctx, "fs_minmax", stream, fs_minmax<true><<<grid, 256, 0, stream>>>(in, n, fs->d_pmin.ptr, fs->d_pmax.ptr, fs->d_psum.ptr));
+	else KL(ctx, "fs_minmax", stream, fs_minmax<false><<<grid, 256, 0, stream>>>(in, n, fs->d_pmin.ptr, fs->d_pmax.ptr, fs->d_psum.ptr));
+	KL(ctx, "fs_autogain_iir", stream, fs_autogain_iir<<<1, 256, 0, stream>>>(in, n, nframes, chunks, fs->d_pmin.ptr, fs->d_pmax.ptr, fs->d_psum.ptr, snr, norm, fs->d_state.ptr, fs->d_params.ptr,
+	                                                                         clip ? fs->d_levels.ptr : NULL));
 	if (!out) return TSDRGPU_OK;                     // statistics only: the caller fuses the normalisation elsewhere
 	const unsigned gx = grid_for(n, ctx->sm_count, 4);
 	dim3 grid2(snr ? (gx < (unsigned) FS_MM_CHUNKS ? gx : FS_MM_CHUNKS) : gx, nframes);
-	if (snr) KL(ctx, "fs_normalise", stream, fs_normalise<true><<<grid2, 256, 0, stream>>>(in, out, n, fs->d_params, fs->d_psq, fs->d_plin));
-	else KL(ctx, "fs_normalise", stream, fs_normalise<false><<<grid2, 256, 0, stream>>>(in, out, n, fs->d_params, fs->d_psq, fs->d_plin));
-	if (snr) KL(ctx, "fs_snr_finish", stream, fs_snr_finish<<<1, 256, 0, stream>>>(nframes, (int) grid2.x, n, fs->d_psq, fs->d_plin, fs->d_params, fs->d_state));
+	if (snr) KL(ctx, "fs_normalise", stream, fs_normalise<true><<<grid2, 256, 0, stream>>>(in, out, n, fs->d_params.ptr, fs->d_psq.ptr, fs->d_plin.ptr));
+	else KL(ctx, "fs_normalise", stream, fs_normalise<false><<<grid2, 256, 0, stream>>>(in, out, n, fs->d_params.ptr, fs->d_psq.ptr, fs->d_plin.ptr));
+	if (snr) KL(ctx, "fs_snr_finish", stream, fs_snr_finish<<<1, 256, 0, stream>>>(nframes, (int) grid2.x, n, fs->d_psq.ptr, fs->d_plin.ptr, fs->d_params.ptr, fs->d_state.ptr));
 	return TSDRGPU_OK;
 }
 
 extern "C" {
 
-int tsdrgpu_framestage_create(tsdrgpu_ctx_t *ctx, tsdrgpu_framestage_t **out) {
-	BIND(ctx); ARG_TRY(ctx, out != NULL);
-	tsdrgpu_framestage *fs = new tsdrgpu_framestage();
-	memset(fs, 0, sizeof(*fs));
-	fs->ctx = ctx;
-	tsdrgpu_gauss_taps(fs->taps);
-	CU_TRY(ctx, cudaMalloc(&fs->d_state, sizeof(SyncState)));
-	CU_TRY(ctx, cudaMalloc(&fs->d_chain, sizeof(double) * 10 * FS_MAX_STRIP));
-	CU_TRY(ctx, cudaMalloc(&fs->d_resume, 256));
-	CU_TRY(ctx, cudaMemset(fs->d_resume, 0, 256));
+// a frame stage whole or half built: its stream and events (null ones are skipped), then the object; its buffers go with it
+static void release(tsdrgpu_framestage *fs) {
+	if (fs->s_side) cudaStreamDestroy(fs->s_side);
+	for (cudaEvent_t e : {fs->ev_ready[0], fs->ev_ready[1], fs->ev_done[0], fs->ev_done[1]}) if (e) cudaEventDestroy(e);
+	delete fs;
+}
+
+static int create_handles(tsdrgpu_framestage *fs) {
+	tsdrgpu_ctx_t *ctx = fs->ctx;
+	CU_TRY(ctx, fs->d_state.assign(1));
+	CU_TRY(ctx, fs->d_chain.assign(10 * FS_MAX_STRIP));
+	CU_TRY(ctx, fs->d_resume.assign(64));
+	CU_TRY(ctx, cudaMemset(fs->d_resume.ptr, 0, 256));
 	{   // highest priority: its single CTA should be placed as soon as an SM has room, ahead of the main stream's queued CTAs
 		int lo = 0, hi = 0;
 		CU_TRY(ctx, cudaDeviceGetStreamPriorityRange(&lo, &hi));
@@ -1476,22 +1478,25 @@ int tsdrgpu_framestage_create(tsdrgpu_ctx_t *ctx, tsdrgpu_framestage_t **out) {
 		CU_TRY(ctx, cudaEventCreateWithFlags(&fs->ev_ready[i], cudaEventDisableTiming));
 		CU_TRY(ctx, cudaEventCreateWithFlags(&fs->ev_done[i], cudaEventDisableTiming));
 	}
-	*out = fs;
 	return tsdrgpu_framestage_reset(fs, NULL);
+}
+
+int tsdrgpu_framestage_create(tsdrgpu_ctx_t *ctx, tsdrgpu_framestage_t **out) {
+	BIND(ctx); ARG_TRY(ctx, out != NULL);
+	tsdrgpu_framestage *fs = new tsdrgpu_framestage();      // value-initialised: every field not set here starts at zero
+	fs->ctx = ctx;
+	tsdrgpu_gauss_taps(fs->taps);
+	const int rc = create_handles(fs);
+	if (rc) { release(fs); return rc; }
+	*out = fs;
+	return TSDRGPU_OK;
 }
 
 void tsdrgpu_framestage_destroy(tsdrgpu_framestage_t *fs) {
 	if (!fs) return;
 	cudaSetDevice(fs->ctx->device);
 	cudaDeviceSynchronize();
-	void *ptrs[] = {fs->d_screen, fs->d_state, fs->d_t1, fs->d_t2[0], fs->d_t2[1], fs->d_wstrips[0], fs->d_wstrips[1], fs->d_hstrips[0],
-	                fs->d_hstrips[1], fs->d_pmin, fs->d_pmax, fs->d_psum, fs->d_psq, fs->d_plin, fs->d_params, fs->d_results[0],
-	                fs->d_results[1], fs->d_chain, fs->d_prep, fs->d_resume, fs->d_sel_hist, fs->d_sel, fs->d_levels};
-	for (void *p : ptrs) if (p) cudaFree(p);
-	enhance_free(&fs->enh);
-	cudaStreamDestroy(fs->s_side);
-	for (int i = 0; i < 2; i++) { cudaEventDestroy(fs->ev_ready[i]); cudaEventDestroy(fs->ev_done[i]); }
-	delete fs;
+	release(fs);
 }
 
 int tsdrgpu_framestage_reset(tsdrgpu_framestage_t *fs, void *stream) {
@@ -1500,10 +1505,14 @@ int tsdrgpu_framestage_reset(tsdrgpu_framestage_t *fs, void *stream) {
 	CU_TRY(fs->ctx, cudaStreamSynchronize(fs->s_side));
 	SyncState s; memset(&s, 0, sizeof s);
 	s.snr = 1.0f;                                        // dsp_autogain_init (dsp.c:35-39)
-	CU_TRY(fs->ctx, cudaMemcpyAsync(fs->d_state, &s, sizeof s, cudaMemcpyHostToDevice, (cudaStream_t) stream));
+	CU_TRY(fs->ctx, cudaMemcpyAsync(fs->d_state.ptr, &s, sizeof s, cudaMemcpyHostToDevice, (cudaStream_t) stream));
 	CU_TRY(fs->ctx, cudaStreamSynchronize((cudaStream_t) stream));
-	if (fs->d_screen) { CU_TRY(fs->ctx, cudaFree(fs->d_screen)); fs->d_screen = NULL; }
-	fs->screen_cap = 0; fs->w = 0; fs->h = 0; fs->n = 0; fs->lp_before_sync = 0; fs->runs = 0; fs->side_pending = 0;
+	{   // the screen buffer goes with `old` (DeviceBuf frees only in its destructor); the next run allocates and zeroes one of its
+		// geometry.  Like every free in a destructor, an error of this one is not reported: nothing is left to recover.
+		DeviceBuf<float> old;
+		fs_exchange(old, fs->d_screen);
+	}
+	fs->w = 0; fs->h = 0; fs->n = 0; fs->lp_before_sync = 0; fs->runs = 0; fs->side_pending = 0;
 	return TSDRGPU_OK;
 }
 
@@ -1572,27 +1581,32 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 	// buffer (re)sizing exactly as dsp.c:152-186
 	if (h != fs->h || w != fs->w) {
 		if ((rc = tsdrgpu_framestage_join(fs, stream))) return rc;
-		fs->h = h; fs->w = w; fs->n = n;
-		if (n > fs->screen_cap) {
-			float *nb;
+		if (n > fs->d_screen.cap) {
 			CU_TRY(ctx, cudaStreamSynchronize(stream));
-			CU_TRY(ctx, cudaMalloc(&nb, sizeof(float) * n));
-			if (fs->d_screen) CU_TRY(ctx, cudaFree(fs->d_screen));
-			fs->d_screen = nb; fs->screen_cap = n;
-			CU_TRY(ctx, cudaMemsetAsync(fs->d_screen, 0, sizeof(float) * n, stream));
+			{   // the new buffer first, then the old one goes with `nb`: a failed allocation leaves the old buffer and the geometry it
+				// was made for in place, so the next call either keeps using both or tries the new geometry again
+				DeviceBuf<float> nb;
+				CU_TRY(ctx, nb.assign(n));
+				fs_exchange(nb, fs->d_screen);
+			}
+			CU_TRY(ctx, cudaMemsetAsync(fs->d_screen.ptr, 0, sizeof(float) * n, stream));
 		}
+		fs->h = h; fs->w = w; fs->n = n;
 	}
 	if (fs->lp_before_sync != (int) lpbs) {
 		if ((rc = tsdrgpu_framestage_join(fs, stream))) return rc;
 		fs->lp_before_sync = lpbs;
-		CU_TRY(ctx, cudaMemsetAsync(fs->d_screen, 0, sizeof(float) * n, stream));
+		CU_TRY(ctx, cudaMemsetAsync(fs->d_screen.ptr, 0, sizeof(float) * n, stream));
 	}
-	if (fs->t_cap < (size_t) nframes * n || fs->batch_cap < nframes) { if ((rc = tsdrgpu_framestage_join(fs, stream))) return rc; }
+	const size_t tneed = (size_t) nframes * n;          // fs_reserve reallocates the group of d_t1 and d_t2 when any of them is short
+	if (fs->d_t1.cap < tneed || fs->d_t2[0].cap < tneed || fs->d_t2[1].cap < tneed || fs->batch_cap < nframes) {
+		if ((rc = tsdrgpu_framestage_join(fs, stream))) return rc;
+	}
 	if ((rc = fs_reserve(fs, nframes, n, w, h))) return rc;
 
 	const int ph = fs->phase; fs->phase ^= 1;
-	float *T2 = fs->d_t2[ph];
-	tsdrgpu_frame_result_t *d_results = fs->d_results[ph];
+	float *T2 = fs->d_t2[ph].ptr;
+	tsdrgpu_frame_result_t *d_results = fs->d_results[ph].ptr;
 	const double fresh = 1.0 - (double) motionblur;      // dsp.c:29
 	const int minsize_x = (int) (w * 0.05f), minsize_y = (int) (h * 0.01f);   // syncdetector.c:178-179
 	const size_t prep_smem = sizeof(double) * ((size_t) w + h + 2);
@@ -1607,17 +1621,17 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 
 	// collapse on `stream`, then sync search on `s2` (== stream unless overlapped)
 	auto collapse_sync = [&](const float *src, cudaStream_t s2) -> int {
-		if ((rc = launch_collapse(ctx, stream, src, w, h, nframes, fs->d_wstrips[ph], fs->d_hstrips[ph], fs->collapse_maps, 4))) return rc;
+		if ((rc = launch_collapse(ctx, stream, src, w, h, nframes, fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, fs->collapse_maps, 4))) return rc;
 		if (s2 != stream) {
 			CU_TRY(ctx, cudaEventRecord(fs->ev_ready[ph], stream));
 			CU_TRY(ctx, cudaStreamWaitEvent(s2, fs->ev_ready[ph], 0));
 		}
 		static const bool no_spec = getenv("TSDRGPU_SYNC_NO_SPEC") != NULL;      // test hook: always the literal cluster search
-		KL(ctx, "fs_sync_prep", s2, fs_sync_prep<<<nframes, FS_SYNC_THREADS, prep_smem, s2>>>(fs->d_wstrips[ph], fs->d_hstrips[ph], w, h,
-			fs->taps[0], fs->taps[1], fs->taps[2], fs->taps[3], fs->taps[4], force_serial, fs->d_prep, fs->d_state, minsize_x, minsize_y, no_spec ? 0 : 1));
-		KL(ctx, "fs_sync_walk", s2, fs_sync_walk<<<1, 64, 0, s2>>>(fs->d_prep, w, h, minsize_x, minsize_y, nframes, fs->d_state, d_results, fs->d_resume));
-		KL(ctx, "fs_sync", s2, fs_sync<<<FS_SEL_CLUSTER, FS_SEL_THREADS, sync_smem, s2>>>(fs->d_prep, sync_nbuf, w, h, minsize_x, minsize_y, nframes,
-			fs->d_state, fs->d_chain, d_results, fs->d_resume));
+		KL(ctx, "fs_sync_prep", s2, fs_sync_prep<<<nframes, FS_SYNC_THREADS, prep_smem, s2>>>(fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, w, h,
+			fs->taps[0], fs->taps[1], fs->taps[2], fs->taps[3], fs->taps[4], force_serial, fs->d_prep.ptr, fs->d_state.ptr, minsize_x, minsize_y, no_spec ? 0 : 1));
+		KL(ctx, "fs_sync_walk", s2, fs_sync_walk<<<1, 64, 0, s2>>>(fs->d_prep.ptr, w, h, minsize_x, minsize_y, nframes, fs->d_state.ptr, d_results, fs->d_resume.ptr));
+		KL(ctx, "fs_sync", s2, fs_sync<<<FS_SEL_CLUSTER, FS_SEL_THREADS, sync_smem, s2>>>(fs->d_prep.ptr, sync_nbuf, w, h, minsize_x, minsize_y, nframes,
+			fs->d_state.ptr, fs->d_chain.ptr, d_results, fs->d_resume.ptr));
 		return TSDRGPU_OK;
 	};
 	// syncdetector_run's output stage: src -> dst (dst != src), or in place on src when allowed
@@ -1648,40 +1662,40 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 		static const bool no_fuse = getenv("TSDRGPU_NO_FUSE") != NULL;
 		const bool fuse = !aap && !snr && nframes <= 4096 && !no_fuse;
 		if (!aap) {
-			if ((rc = fs_autogain_batch(fs, stream, d_in, fuse ? NULL : fs->d_t1, nframes, n, lowpasscoeff, snr))) return rc;
-			lp_in = fs->d_t1;
-			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
+			if ((rc = fs_autogain_batch(fs, stream, d_in, fuse ? NULL : fs->d_t1.ptr, nframes, n, lowpasscoeff, snr))) return rc;
+			lp_in = fs->d_t1.ptr;
+			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
 		}
 		if (fuse) {
 			// one thread per four pixels on the 16-byte path, one per pixel otherwise (odd frame sizes, unaligned input)
-			const bool vec = ((n & 3) == 0) && (((reinterpret_cast<unsigned long long>(d_in) | reinterpret_cast<unsigned long long>(T2) | reinterpret_cast<unsigned long long>(fs->d_screen)) & 15ull) == 0);
+			const bool vec = ((n & 3) == 0) && (((reinterpret_cast<unsigned long long>(d_in) | reinterpret_cast<unsigned long long>(T2) | reinterpret_cast<unsigned long long>(fs->d_screen.ptr)) & 15ull) == 0);
 			const size_t threads = vec ? n / 4 : n;
 			const unsigned grid = (unsigned) ((threads + 255) / 256 ? (threads + 255) / 256 : 1);
-			if (vec) KL(ctx, "fs_norm_lowpass", stream, fs_norm_lowpass<true><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen, n, nframes, fs->d_params, motionblur, fresh));
-			else KL(ctx, "fs_norm_lowpass", stream, fs_norm_lowpass<false><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen, n, nframes, fs->d_params, motionblur, fresh));
+			if (vec) KL(ctx, "fs_norm_lowpass", stream, fs_norm_lowpass<true><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh));
+			else KL(ctx, "fs_norm_lowpass", stream, fs_norm_lowpass<false><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh));
 		}
-		else KL(ctx, "fs_timelowpass", stream, fs_timelowpass<<<gx, 256, 0, stream>>>(lp_in, T2, fs->d_screen, n, nframes, motionblur, fresh));
+		else KL(ctx, "fs_timelowpass", stream, fs_timelowpass<<<gx, 256, 0, stream>>>(lp_in, T2, fs->d_screen.ptr, n, nframes, motionblur, fresh));
 		if (overlapped) tail = fs->s_side;
 		if ((rc = collapse_sync(T2, tail))) return rc;
-		float *dst = aap ? fs->d_t1 : d_out;
+		float *dst = aap ? fs->d_t1.ptr : d_out;
 		if ((rc = emit(T2, dst, !superres, false, &res, tail))) return rc;
 		if (aap) {
 			if ((rc = fs_autogain_batch(fs, stream, res, d_out, nframes, n, lowpasscoeff, snr))) return rc;
-			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
+			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
 		} else if (res != d_out && (rc = fs_copy_async(ctx, tail, res, d_out, total))) return rc;
 	} else {                                             // dsp.c:214-226
-		float *work = fs->d_t1;
+		float *work = fs->d_t1.ptr;
 		if (!aap) {
-			if ((rc = fs_autogain_batch(fs, stream, d_in, fs->d_t1, nframes, n, lowpasscoeff, snr))) return rc;
-			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
-		} else if ((rc = fs_copy_async(ctx, stream, d_in, fs->d_t1, total))) return rc;
+			if ((rc = fs_autogain_batch(fs, stream, d_in, fs->d_t1.ptr, nframes, n, lowpasscoeff, snr))) return rc;
+			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
+		} else if ((rc = fs_copy_async(ctx, stream, d_in, fs->d_t1.ptr, total))) return rc;
 		if ((rc = collapse_sync(work, stream))) return rc;
 		if ((rc = emit(work, T2, (motionblur == 0.0f) && !superres, true, &res, stream))) return rc;
-		float *lp_out = aap ? ((res == fs->d_t1) ? T2 : fs->d_t1) : d_out;
-		KL(ctx, "fs_timelowpass", stream, fs_timelowpass<<<gx, 256, 0, stream>>>(res, lp_out, fs->d_screen, n, nframes, motionblur, fresh));
+		float *lp_out = aap ? ((res == fs->d_t1.ptr) ? T2 : fs->d_t1.ptr) : d_out;
+		KL(ctx, "fs_timelowpass", stream, fs_timelowpass<<<gx, 256, 0, stream>>>(res, lp_out, fs->d_screen.ptr, n, nframes, motionblur, fresh));
 		if (aap) {
 			if ((rc = fs_autogain_batch(fs, stream, lp_out, d_out, nframes, n, lowpasscoeff, snr))) return rc;
-			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params, fs->d_state, d_results));
+			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
 		}
 	}
 	// NLM, then CLAHE, on the frames as delivered, after every branch's last step; nothing either does feeds back
@@ -1723,12 +1737,12 @@ int tsdrgpu_autogain(tsdrgpu_ctx_t *ctx, void *stream_, float *h_lastmax, float 
 	if (rc) return rc;
 	SyncState s; memset(&s, 0, sizeof s);
 	s.lastmax = *h_lastmax; s.lastmin = *h_lastmin; s.snr = h_snr ? *h_snr : 1.0f;
-	CU_TRY(ctx, cudaMemcpy(fs->d_state, &s, sizeof s, cudaMemcpyHostToDevice));
+	CU_TRY(ctx, cudaMemcpy(fs->d_state.ptr, &s, sizeof s, cudaMemcpyHostToDevice));
 	if ((rc = fs_reserve(fs, 1, 1, 1, 1))) { tsdrgpu_framestage_destroy(fs); return rc; }
 	rc = fs_autogain_batch(fs, stream, d_in, d_out, 1, (size_t) n, norm, h_snr != NULL);
 	if (rc == TSDRGPU_OK) {
 		CU_TRY(ctx, cudaStreamSynchronize(stream));
-		CU_TRY(ctx, cudaMemcpy(&s, fs->d_state, sizeof s, cudaMemcpyDeviceToHost));
+		CU_TRY(ctx, cudaMemcpy(&s, fs->d_state.ptr, sizeof s, cudaMemcpyDeviceToHost));
 		*h_lastmax = s.lastmax; *h_lastmin = s.lastmin; if (h_snr) *h_snr = s.snr;
 	}
 	tsdrgpu_framestage_destroy(fs);
@@ -1746,15 +1760,14 @@ int tsdrgpu_frame_levels(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_frame
 	int rc = tsdrgpu_framestage_create(ctx, &fs);
 	if (rc) return rc;
 	if (!(rc = fs_reserve(fs, nframes, 1, 1, 1)) && !(rc = fs_select_batch(fs, stream, d_frames, nframes, (size_t) n, ppm, fs_chunks((size_t) n), false))) {
-		float2 *lv = (float2 *) malloc(sizeof(float2) * nframes);
-		SelState *st = (SelState *) malloc(sizeof(SelState) * nframes);
-		cudaError_t e = cudaMemcpyAsync(lv, fs->d_levels, sizeof(float2) * nframes, cudaMemcpyDeviceToHost, stream);
-		if (e == cudaSuccess) e = cudaMemcpyAsync(st, fs->d_sel, sizeof(SelState) * nframes, cudaMemcpyDeviceToHost, stream);
+		std::vector<float2> lv(nframes);
+		std::vector<SelState> st(nframes);
+		cudaError_t e = cudaMemcpyAsync(lv.data(), fs->d_levels.ptr, sizeof(float2) * nframes, cudaMemcpyDeviceToHost, stream);
+		if (e == cudaSuccess) e = cudaMemcpyAsync(st.data(), fs->d_sel.ptr, sizeof(SelState) * nframes, cudaMemcpyDeviceToHost, stream);
 		if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
 		if (e == cudaSuccess) {
 			for (int f = 0; f < nframes; f++) { h_lo[f] = lv[f].x; h_hi[f] = lv[f].y; if (h_valid) h_valid[f] = st[f].nvalid; }
 		} else rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "tsdrgpu_frame_levels", e, __FILE__, __LINE__);
-		free(lv); free(st);
 	}
 	tsdrgpu_framestage_destroy(fs);
 	return rc;

@@ -558,16 +558,16 @@ __global__ void __launch_bounds__(256) demod_kernel(const float2 *__restrict__ i
 struct tsdrgpu_resampler {
 	tsdrgpu_ctx_t *ctx;
 	double offset;             // host: data-independent phase state (dsp_resample_t.offset)
-	double *d_contrib;         // device: dsp_resample_t.contrib
-	// descriptor staging: pinned ring + device copies, one slot per in-flight run
+	DeviceBuf<double> d_contrib;                        // device: dsp_resample_t.contrib
+	// descriptor staging: pinned ring + device copies (bytes), one slot per in-flight run
 	static constexpr int SLOTS = 4;
-	void *h_desc[SLOTS]; void *d_desc[SLOTS]; size_t desc_bytes[SLOTS]; cudaEvent_t ev[SLOTS]; int next;
-	double *d_bank; int *d_has_a; size_t bank_cap;
+	PinnedBuf<unsigned char> h_desc[SLOTS]; DeviceBuf<unsigned char> d_desc[SLOTS]; cudaEvent_t ev[SLOTS]; int next;
+	DeviceBuf<double> d_bank; DeviceBuf<int> d_has_a;
 	float *d_mag_next;         // one-shot: the next IQ run also writes the magnitudes here (tsdrgpu_resampler_set_mag_out)
 	// windowed-sinc mode (tsdrgpu_resampler_set_kernel)
 	int kernel;                // TSDRGPU_RS_BOX / TSDRGPU_RS_SINC
-	float *d_hist[2]; int hist_cur; int hist_zero;      // last H magnitudes: runs read d_hist[hist_cur], write the other; zero before the next run
-	float *d_taps; double taps_fc;                      // tap table on the device, built for min(1, r) == taps_fc (0: none yet)
+	DeviceBuf<float> d_hist[2]; int hist_cur; int hist_zero;      // last H magnitudes: runs read d_hist[hist_cur], write the other; zero before the next run
+	DeviceBuf<float> d_taps; double taps_fc;            // tap table on the device, built for min(1, r) == taps_fc (0: none yet)
 };
 
 extern "C" {
@@ -582,19 +582,31 @@ int tsdrgpu_am_demod(tsdrgpu_ctx_t *ctx, void *stream, const float *d_iq, uint64
 	return TSDRGPU_OK;
 }
 
+// a resampler whole or half built: its events (null ones are skipped), then the object; its buffers go with it
+static void release(tsdrgpu_resampler *r) {
+	for (cudaEvent_t e : r->ev) if (e) cudaEventDestroy(e);
+	delete r;
+}
+
+static int create_handles(tsdrgpu_resampler *r) {
+	tsdrgpu_ctx_t *ctx = r->ctx;
+	CU_TRY(ctx, r->d_contrib.assign(1));
+	CU_TRY(ctx, cudaMemset(r->d_contrib.ptr, 0, sizeof(double)));
+	for (cudaEvent_t &e : r->ev) CU_TRY(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+	for (DeviceBuf<float> &h : r->d_hist) {
+		CU_TRY(ctx, h.assign(SINC_H));
+		CU_TRY(ctx, cudaMemset(h.ptr, 0, sizeof(float) * SINC_H));
+	}
+	CU_TRY(ctx, r->d_taps.assign(SINC_T * SINC_L));
+	return TSDRGPU_OK;
+}
+
 int tsdrgpu_resampler_create(tsdrgpu_ctx_t *ctx, tsdrgpu_resampler_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
-	tsdrgpu_resampler *r = new tsdrgpu_resampler();
-	memset(r, 0, sizeof(*r));
+	tsdrgpu_resampler *r = new tsdrgpu_resampler();      // value-initialised: every field not set here starts at zero
 	r->ctx = ctx;
-	CU_TRY(ctx, cudaMalloc(&r->d_contrib, sizeof(double)));
-	CU_TRY(ctx, cudaMemset(r->d_contrib, 0, sizeof(double)));
-	for (int i = 0; i < tsdrgpu_resampler::SLOTS; i++) CU_TRY(ctx, cudaEventCreateWithFlags(&r->ev[i], cudaEventDisableTiming));
-	for (int i = 0; i < 2; i++) {
-		CU_TRY(ctx, cudaMalloc(&r->d_hist[i], sizeof(float) * SINC_H));
-		CU_TRY(ctx, cudaMemset(r->d_hist[i], 0, sizeof(float) * SINC_H));
-	}
-	CU_TRY(ctx, cudaMalloc(&r->d_taps, sizeof(float) * SINC_T * SINC_L));
+	const int rc = create_handles(r);
+	if (rc) { release(r); return rc; }
 	*out = r;
 	return TSDRGPU_OK;
 }
@@ -603,16 +615,7 @@ void tsdrgpu_resampler_destroy(tsdrgpu_resampler_t *r) {
 	if (!r) return;
 	cudaSetDevice(r->ctx->device);
 	cudaDeviceSynchronize();
-	cudaFree(r->d_contrib);
-	for (int i = 0; i < tsdrgpu_resampler::SLOTS; i++) {
-		if (r->h_desc[i]) cudaFreeHost(r->h_desc[i]);
-		if (r->d_desc[i]) cudaFree(r->d_desc[i]);
-		cudaEventDestroy(r->ev[i]);
-	}
-	if (r->d_bank) cudaFree(r->d_bank);
-	if (r->d_has_a) cudaFree(r->d_has_a);
-	cudaFree(r->d_hist[0]); cudaFree(r->d_hist[1]); cudaFree(r->d_taps);
-	delete r;
+	release(r);
 }
 
 int tsdrgpu_resampler_set_kernel(tsdrgpu_resampler_t *r, int kernel) {
@@ -633,8 +636,8 @@ int tsdrgpu_resampler_reset(tsdrgpu_resampler_t *r, void *stream) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, r != NULL);
 	BIND(r->ctx);
 	r->offset = 0.0;
-	CU_TRY(r->ctx, cudaMemsetAsync(r->d_contrib, 0, sizeof(double), (cudaStream_t) stream));
-	CU_TRY(r->ctx, cudaMemsetAsync(r->d_hist[r->hist_cur], 0, sizeof(float) * SINC_H, (cudaStream_t) stream));
+	CU_TRY(r->ctx, cudaMemsetAsync(r->d_contrib.ptr, 0, sizeof(double), (cudaStream_t) stream));
+	CU_TRY(r->ctx, cudaMemsetAsync(r->d_hist[r->hist_cur].ptr, 0, sizeof(float) * SINC_H, (cudaStream_t) stream));
 	r->hist_zero = 0;
 	return TSDRGPU_OK;
 }
@@ -643,7 +646,7 @@ int tsdrgpu_resampler_get_state(tsdrgpu_resampler_t *r, void *stream, double *co
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, r != NULL);
 	BIND(r->ctx);
 	if (contrib) {
-		CU_TRY(r->ctx, cudaMemcpyAsync(contrib, r->d_contrib, sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t) stream));
+		CU_TRY(r->ctx, cudaMemcpyAsync(contrib, r->d_contrib.ptr, sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t) stream));
 		CU_TRY(r->ctx, cudaStreamSynchronize((cudaStream_t) stream));
 	}
 	if (offset) *offset = r->offset;
@@ -654,7 +657,7 @@ int tsdrgpu_resampler_set_state(tsdrgpu_resampler_t *r, void *stream, double con
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, r != NULL);
 	BIND(r->ctx);
 	r->offset = offset;
-	CU_TRY(r->ctx, cudaMemcpyAsync(r->d_contrib, &contrib, sizeof(double), cudaMemcpyHostToDevice, (cudaStream_t) stream));
+	CU_TRY(r->ctx, cudaMemcpyAsync(r->d_contrib.ptr, &contrib, sizeof(double), cudaMemcpyHostToDevice, (cudaStream_t) stream));
 	CU_TRY(r->ctx, cudaStreamSynchronize((cudaStream_t) stream));
 	return TSDRGPU_OK;
 }
@@ -695,15 +698,12 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 	const size_t need = sizeof(tsdrgpu_rs_block_t) * nblocks + sizeof(uint2) * (max_tiles + 1);
 	const int slot = r->next; r->next = (r->next + 1) % tsdrgpu_resampler::SLOTS;
 	CU_TRY(ctx, cudaEventSynchronize(r->ev[slot]));
-	if (r->desc_bytes[slot] < need) {
-		if (r->h_desc[slot]) CU_TRY(ctx, cudaFreeHost(r->h_desc[slot]));
-		if (r->d_desc[slot]) CU_TRY(ctx, cudaFree(r->d_desc[slot]));
-		const size_t cap = need * 2;
-		CU_TRY(ctx, cudaMallocHost(&r->h_desc[slot], cap));
-		CU_TRY(ctx, cudaMalloc(&r->d_desc[slot], cap));
-		r->desc_bytes[slot] = cap;
+	if (r->h_desc[slot].cap < need || r->d_desc[slot].cap < need) {
+		const int rc = r->h_desc[slot].assign(ctx, need * 2);
+		if (rc) return rc;
+		CU_TRY(ctx, r->d_desc[slot].assign(need * 2));
 	}
-	tsdrgpu_rs_block_t *hb = (tsdrgpu_rs_block_t *) r->h_desc[slot];
+	tsdrgpu_rs_block_t *hb = (tsdrgpu_rs_block_t *) r->h_desc[slot].ptr;
 	uint2 *hp = (uint2 *) (hb + nblocks);
 
 	double off = r->offset;
@@ -731,9 +731,9 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 		for (unsigned s0 = 0; s0 < hb[b].size; s0 = (s0 == 0) ? RS_TILE - lead : s0 + RS_TILE) hp[tiles++] = make_uint2(b, s0);
 		if (hb[b].n_out > max_out) max_out = hb[b].n_out;
 	}
-	CU_TRY(ctx, cudaMemcpyAsync(r->d_desc[slot], r->h_desc[slot], need, cudaMemcpyHostToDevice, stream));
+	CU_TRY(ctx, cudaMemcpyAsync(r->d_desc[slot].ptr, r->h_desc[slot].ptr, need, cudaMemcpyHostToDevice, stream));
 	CU_TRY(ctx, cudaEventRecord(r->ev[slot], stream));
-	const RsBlock *db = (const RsBlock *) r->d_desc[slot];
+	const RsBlock *db = (const RsBlock *) r->d_desc[slot].ptr;
 	const uint2 *dp = (const uint2 *) (db + nblocks);
 
 	float *mag = r->d_mag_next; r->d_mag_next = NULL;
@@ -743,15 +743,15 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 		if (r->taps_fc != fc) {                           // pageable source: the copy is staged before the call returns
 			static thread_local float h_taps[SINC_T * SINC_L];
 			tsdrgpu_sinc_taps(ratio, h_taps, NULL, NULL);
-			CU_TRY(ctx, cudaMemcpyAsync(r->d_taps, h_taps, sizeof h_taps, cudaMemcpyHostToDevice, stream));
+			CU_TRY(ctx, cudaMemcpyAsync(r->d_taps.ptr, h_taps, sizeof h_taps, cudaMemcpyHostToDevice, stream));
 			r->taps_fc = fc;
 		}
-		if (r->hist_zero) { CU_TRY(ctx, cudaMemsetAsync(r->d_hist[r->hist_cur], 0, sizeof(float) * SINC_H, stream)); r->hist_zero = 0; }
+		if (r->hist_zero) { CU_TRY(ctx, cudaMemsetAsync(r->d_hist[r->hist_cur].ptr, 0, sizeof(float) * SINC_H, stream)); r->hist_zero = 0; }
 		uint64_t run_samples = 0;
 		for (uint32_t b = 0; b < nblocks; b++) run_samples += hb[b].size;
-		const float *hin = r->d_hist[r->hist_cur];
-		float *hout = r->d_hist[r->hist_cur ^ 1];
-		const float4 *taps = reinterpret_cast<const float4 *>(r->d_taps);
+		const float *hin = r->d_hist[r->hist_cur].ptr;
+		float *hout = r->d_hist[r->hist_cur ^ 1].ptr;
+		const float4 *taps = reinterpret_cast<const float4 *>(r->d_taps.ptr);
 		if (in_is_iq) KL(ctx, "rs_sinc", stream, rs_sinc<true><<<tiles, SINC_THREADS, 0, stream>>>(d_in, d_out, db, dp, sinc_pt, taps, hin, hout, run_samples, mag));
 		else KL(ctx, "rs_sinc", stream, rs_sinc<false><<<tiles, SINC_THREADS, 0, stream>>>(d_in, d_out, db, dp, sinc_pt, taps, hin, hout, run_samples, (float *) NULL));
 		r->hist_cur ^= 1;
@@ -760,11 +760,10 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 		if (in_is_iq) KL(ctx, "rs_nearest", stream, rs_nearest<true><<<grid, 256, 0, stream>>>(d_in, d_out, db));
 		else KL(ctx, "rs_nearest", stream, rs_nearest<false><<<grid, 256, 0, stream>>>(d_in, d_out, db));
 	} else {
-		if (r->bank_cap < (size_t) nblocks + 1) {
-			if (r->d_bank) { CU_TRY(ctx, cudaStreamSynchronize(stream)); CU_TRY(ctx, cudaFree(r->d_bank)); CU_TRY(ctx, cudaFree(r->d_has_a)); }
-			r->bank_cap = (size_t) nblocks * 2 + 2;
-			CU_TRY(ctx, cudaMalloc(&r->d_bank, sizeof(double) * r->bank_cap));
-			CU_TRY(ctx, cudaMalloc(&r->d_has_a, sizeof(int) * r->bank_cap));
+		if (r->d_bank.cap < (size_t) nblocks + 1 || r->d_has_a.cap < (size_t) nblocks + 1) {
+			if (r->d_bank.ptr || r->d_has_a.ptr) CU_TRY(ctx, cudaStreamSynchronize(stream));
+			CU_TRY(ctx, r->d_bank.assign((size_t) nblocks * 2 + 2));
+			CU_TRY(ctx, r->d_has_a.assign((size_t) nblocks * 2 + 2));
 		}
 		if (v1) {
 			if (in_is_iq) KL(ctx, "rs_main", stream, rs_main<true><<<tiles, RS_THREADS, 0, stream>>>(d_in, d_out, db, dp, mag));
@@ -781,8 +780,8 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 				else KL(ctx, "rs_main", stream, rs_main4<true, 3><<<tiles, RS_THREADS, 0, stream>>>(d_in, d_out, db, dp, mag));
 			} else KL(ctx, "rs_main", stream, rs_main4<false, 5><<<tiles, RS_THREADS, 0, stream>>>(d_in, d_out, db, dp, (float *) NULL));
 		}
-		if (in_is_iq) KL(ctx, "rs_fixup", stream, rs_fixup<true><<<1, 256, 0, stream>>>(d_in, d_out, db, nblocks, r->d_bank, r->d_has_a, r->d_contrib));
-		else KL(ctx, "rs_fixup", stream, rs_fixup<false><<<1, 256, 0, stream>>>(d_in, d_out, db, nblocks, r->d_bank, r->d_has_a, r->d_contrib));
+		if (in_is_iq) KL(ctx, "rs_fixup", stream, rs_fixup<true><<<1, 256, 0, stream>>>(d_in, d_out, db, nblocks, r->d_bank.ptr, r->d_has_a.ptr, r->d_contrib.ptr));
+		else KL(ctx, "rs_fixup", stream, rs_fixup<false><<<1, 256, 0, stream>>>(d_in, d_out, db, nblocks, r->d_bank.ptr, r->d_has_a.ptr, r->d_contrib.ptr));
 	}
 	r->offset = off;
 	if (h_n_out) *h_n_out = total;

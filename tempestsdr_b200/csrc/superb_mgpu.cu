@@ -206,11 +206,11 @@ struct tsdrgpu_superb_mgpu {
 	tsdrgpu_ctx_t *ctx;
 	int H, log2H, rank, root;
 	unsigned n_max;                                   // largest transform length the window was sized for
-	unsigned char *win; size_t win_bytes;
+	DeviceBuf<unsigned char> win;
 	size_t off_d, off_x, off_v, off_r;                // byte offsets in the window: D (difference spectrum), Xp (re-ordered spectrum), A (block transform), the root's stream
 	Peers peers; int connected; int ipc_opened[SBM_MAX_RANKS];
-	float2 *d_work, *d_p, *d_x; void *d_part; int *d_lag;   // local temporaries (d_work, d_dd: 2 n_max complex -- the two difference signals / spectra side by side)
-	float2 *d_dd, *d_side;                            // d_side: the side stream's transform scratch
+	DeviceBuf<float2> d_work, d_p, d_x; DeviceBuf<unsigned char> d_part; DeviceBuf<int> d_lag;   // local temporaries (d_work, d_dd: 2 n_max complex -- the two difference signals / spectra side by side)
+	DeviceBuf<float2> d_dd, d_side;                   // d_side: the side stream's transform scratch
 	cudaStream_t s_side; cudaEvent_t ev_fork, ev_join; // the hop's own spectrum runs beside the lag search
 	unsigned epoch; unsigned last_n;
 	unsigned prep_n, prep_nd;                         // transform sizes whose kernels and twiddle tables are known to be resident
@@ -219,11 +219,40 @@ struct tsdrgpu_superb_mgpu {
 
 extern "C" {
 
+// a group member whole or half built: the peers' windows are unmapped before its own window goes, then its stream and events
+// (null ones are skipped) and the object; its buffers go with it
+static void release(tsdrgpu_superb_mgpu *g) {
+	for (int q = 0; q < g->H; q++) if (g->ipc_opened[q] && g->peers.win[q]) cudaIpcCloseMemHandle(g->peers.win[q]);
+	if (g->s_side) cudaStreamDestroy(g->s_side);
+	if (g->ev_fork) cudaEventDestroy(g->ev_fork);
+	if (g->ev_join) cudaEventDestroy(g->ev_join);
+	delete g;
+}
+
+static int create_handles(tsdrgpu_superb_mgpu *g) {
+	tsdrgpu_ctx_t *ctx = g->ctx;
+	const size_t n = g->n_max;
+	CU_TRY(ctx, g->win.assign(g->off_r + sizeof(float) * n * (size_t) g->H));
+	CU_TRY(ctx, cudaMemset(g->win.ptr, 0, sizeof(WinHeader)));
+	CU_TRY(ctx, g->d_work.assign(2 * n));
+	CU_TRY(ctx, g->d_dd.assign(2 * n));
+	CU_TRY(ctx, g->d_side.assign(n));
+	CU_TRY(ctx, g->d_p.assign(n));
+	CU_TRY(ctx, g->d_x.assign(n));
+	CU_TRY(ctx, cudaStreamCreateWithFlags(&g->s_side, cudaStreamNonBlocking));
+	CU_TRY(ctx, cudaEventCreateWithFlags(&g->ev_fork, cudaEventDisableTiming));
+	CU_TRY(ctx, cudaEventCreateWithFlags(&g->ev_join, cudaEventDisableTiming));
+	CU_TRY(ctx, g->d_part.assign(8 * TSDRGPU_ARGMAX_PARTS));
+	CU_TRY(ctx, g->d_lag.assign(64));
+	CU_TRY(ctx, cudaMemset(g->d_lag.ptr, 0, 256));
+	CU_TRY(ctx, cudaDeviceSynchronize());
+	return TSDRGPU_OK;
+}
+
 int tsdrgpu_superb_mgpu_create(tsdrgpu_ctx_t *ctx, int nranks, int rank, int root, uint32_t max_pairs_per_hop, tsdrgpu_superb_mgpu_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
 	ARG_TRY(ctx, (nranks == 2 || nranks == 4 || nranks == 8 || nranks == 16) && rank >= 0 && rank < nranks && root >= 0 && root < nranks && max_pairs_per_hop >= 64);
-	tsdrgpu_superb_mgpu *g = new tsdrgpu_superb_mgpu();
-	memset(g, 0, sizeof *g);
+	tsdrgpu_superb_mgpu *g = new tsdrgpu_superb_mgpu();      // value-initialised: every field not set here starts at zero
 	g->ctx = ctx; g->H = nranks; g->rank = rank; g->root = root;
 	while ((1 << g->log2H) < nranks) g->log2H++;
 	g->n_max = tsdrgpu_fft_getrealsize(max_pairs_per_hop);
@@ -232,22 +261,9 @@ int tsdrgpu_superb_mgpu_create(tsdrgpu_ctx_t *ctx, int nranks, int rank, int roo
 	g->off_x = g->off_d + sizeof(float2) * n;         // nd <= n
 	g->off_v = g->off_x + sizeof(float2) * n;
 	g->off_r = g->off_v + sizeof(float2) * n;
-	g->win_bytes = g->off_r + sizeof(float) * n * (size_t) nranks;
-	CU_TRY(ctx, cudaMalloc(&g->win, g->win_bytes));
-	CU_TRY(ctx, cudaMemset(g->win, 0, sizeof(WinHeader)));
-	CU_TRY(ctx, cudaMalloc(&g->d_work, sizeof(float2) * 2 * n));
-	CU_TRY(ctx, cudaMalloc(&g->d_dd, sizeof(float2) * 2 * n));
-	CU_TRY(ctx, cudaMalloc(&g->d_side, sizeof(float2) * n));
-	CU_TRY(ctx, cudaMalloc(&g->d_p, sizeof(float2) * n));
-	CU_TRY(ctx, cudaMalloc(&g->d_x, sizeof(float2) * n));
-	CU_TRY(ctx, cudaStreamCreateWithFlags(&g->s_side, cudaStreamNonBlocking));
-	CU_TRY(ctx, cudaEventCreateWithFlags(&g->ev_fork, cudaEventDisableTiming));
-	CU_TRY(ctx, cudaEventCreateWithFlags(&g->ev_join, cudaEventDisableTiming));
-	CU_TRY(ctx, cudaMalloc(&g->d_part, 8 * TSDRGPU_ARGMAX_PARTS));
-	CU_TRY(ctx, cudaMalloc(&g->d_lag, 256));
-	CU_TRY(ctx, cudaMemset(g->d_lag, 0, 256));
-	CU_TRY(ctx, cudaDeviceSynchronize());
-	g->peers.win[rank] = g->win;
+	const int rc = create_handles(g);
+	if (rc) { release(g); return rc; }
+	g->peers.win[rank] = g->win.ptr;
 	const char *to = getenv("TSDRGPU_SBM_TIMEOUT_MS");
 	g->timeout_cycles = (long long) ((to ? atof(to) : 15000.0) * 1.9e6);      // ~1.9 GHz SM clock
 	*out = g;
@@ -272,20 +288,14 @@ void tsdrgpu_superb_mgpu_destroy(tsdrgpu_superb_mgpu_t *g) {
 	if (!g) return;
 	cudaSetDevice(g->ctx->device);
 	cudaDeviceSynchronize();
-	for (int q = 0; q < g->H; q++) if (g->ipc_opened[q] && g->peers.win[q]) cudaIpcCloseMemHandle(g->peers.win[q]);
-	cudaFree(g->win); cudaFree(g->d_work); cudaFree(g->d_p); cudaFree(g->d_x); cudaFree(g->d_part); cudaFree(g->d_lag);
-	cudaFree(g->d_dd); cudaFree(g->d_side);
-	if (g->s_side) cudaStreamDestroy(g->s_side);
-	if (g->ev_fork) cudaEventDestroy(g->ev_fork);
-	if (g->ev_join) cudaEventDestroy(g->ev_join);
-	delete g;
+	release(g);
 }
 
 int tsdrgpu_superb_mgpu_export(tsdrgpu_superb_mgpu_t *g, uint8_t handle[64]) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, g != NULL && handle != NULL);
 	BIND(g->ctx);
 	cudaIpcMemHandle_t h;
-	CU_TRY(g->ctx, cudaIpcGetMemHandle(&h, g->win));
+	CU_TRY(g->ctx, cudaIpcGetMemHandle(&h, g->win.ptr));
 	memcpy(handle, &h, 64);
 	return TSDRGPU_OK;
 }
@@ -324,7 +334,7 @@ int tsdrgpu_superb_mgpu_connect_local(tsdrgpu_superb_mgpu_t *const *all, int nra
 				if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "cudaDeviceEnablePeerAccess", e, __FILE__, __LINE__);
 				cudaGetLastError();
 			}
-			all[r]->peers.win[q] = all[q]->win;
+			all[r]->peers.win[q] = all[q]->win.ptr;
 		}
 		all[r]->connected = 1;
 	}
@@ -343,15 +353,15 @@ static int sbm_prepare(tsdrgpu_superb_mgpu *g, cudaStream_t stream, unsigned N, 
 	if (g->prep_n == N && g->prep_nd == nd) return TSDRGPU_OK;
 	tsdrgpu_ctx_t *ctx = g->ctx;
 	int rc;
-	CU_TRY(ctx, cudaMemsetAsync(g->d_work, 0, sizeof(float2) * N, stream));
-	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work, g->d_x, N, 0))) return rc;
-	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work, g->d_p, nd, 0))) return rc;
-	if ((rc = tsdrgpu_fft_internal(ctx, stream, g->d_p, nd, 1))) return rc;
-	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work, g->d_x, N, 1))) return rc;
-	int *tmp_lag = g->d_lag + 8;
-	if ((rc = tsdrgpu_argmax_mag_internal(ctx, stream, g->d_p, nd, g->d_part, tmp_lag))) return rc;
-	if ((rc = tsdrgpu_fft_batch_internal(ctx, stream, g->d_work, (long long) nd, g->d_dd, (long long) nd, NULL, nd, 2, 0))) return rc;
-	if ((rc = tsdrgpu_fft_batch_internal(ctx, g->s_side, g->d_work, 0, g->d_x, 0, g->d_side, N, 1, 0))) return rc;
+	CU_TRY(ctx, cudaMemsetAsync(g->d_work.ptr, 0, sizeof(float2) * N, stream));
+	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work.ptr, g->d_x.ptr, N, 0))) return rc;
+	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work.ptr, g->d_p.ptr, nd, 0))) return rc;
+	if ((rc = tsdrgpu_fft_internal(ctx, stream, g->d_p.ptr, nd, 1))) return rc;
+	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work.ptr, g->d_x.ptr, N, 1))) return rc;
+	int *tmp_lag = g->d_lag.ptr + 8;
+	if ((rc = tsdrgpu_argmax_mag_internal(ctx, stream, g->d_p.ptr, nd, g->d_part.ptr, tmp_lag))) return rc;
+	if ((rc = tsdrgpu_fft_batch_internal(ctx, stream, g->d_work.ptr, (long long) nd, g->d_dd.ptr, (long long) nd, NULL, nd, 2, 0))) return rc;
+	if ((rc = tsdrgpu_fft_batch_internal(ctx, g->s_side, g->d_work.ptr, 0, g->d_x.ptr, 0, g->d_side.ptr, N, 1, 0))) return rc;
 	CU_TRY(ctx, cudaStreamSynchronize(g->s_side));
 	preload(sbm_abs_diff2);
 	preload(sbm_sync); preload(sbm_abs_diff); preload(sbm_xcorr_pull); preload(sbm_permute_ramp); preload(sbm_pull_blocks);
@@ -388,7 +398,7 @@ int tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stream_, const fl
 	if ((rc = sbm_prepare(g, stream, N, nd))) return rc;
 	const unsigned epoch = ++g->epoch;
 	g->last_n = N;
-	float2 *D = reinterpret_cast<float2 *>(g->win + g->off_d), *Xp = reinterpret_cast<float2 *>(g->win + g->off_x), *Ablk = reinterpret_cast<float2 *>(g->win + g->off_v);
+	float2 *D = reinterpret_cast<float2 *>(g->win.ptr + g->off_d), *Xp = reinterpret_cast<float2 *>(g->win.ptr + g->off_x), *Ablk = reinterpret_cast<float2 *>(g->win.ptr + g->off_v);
 	// ---- phase 1: this hop's spectrum, this hop's alignment lag, the spectrum re-ordered + ramped into the own window
 	// The hop's own spectrum (N points) and the search for its lag (three nd-point transforms) do not depend on each other, and a
 	// single transform of this size fills the chip for little more than one wave of CTAs: on every rank but the first the spectrum
@@ -397,39 +407,39 @@ int tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stream_, const fl
 	if (forked) {
 		CU_TRY(ctx, cudaEventRecord(g->ev_fork, stream));
 		CU_TRY(ctx, cudaStreamWaitEvent(g->s_side, g->ev_fork, 0));
-		if ((rc = tsdrgpu_fft_batch_internal(ctx, g->s_side, reinterpret_cast<const float2 *>(d_hop), 0, g->d_x, 0, g->d_side, N, 1, 0))) return rc;
+		if ((rc = tsdrgpu_fft_batch_internal(ctx, g->s_side, reinterpret_cast<const float2 *>(d_hop), 0, g->d_x.ptr, 0, g->d_side.ptr, N, 1, 0))) return rc;
 		CU_TRY(ctx, cudaEventRecord(g->ev_join, g->s_side));
-	} else if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, reinterpret_cast<const float2 *>(d_hop), g->d_x, N, 0))) return rc;
+	} else if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, reinterpret_cast<const float2 *>(d_hop), g->d_x.ptr, N, 0))) return rc;
 	if (rank != 0) {
 		const float4 *d0;
 		if (d_hop0) {                                         // the alignment reference is resident here: both difference spectra in one batched transform
-			KL(ctx, "sbm_abs_diff", stream, sbm_abs_diff2<<<dim3(grid_for(nd, ctx->sm_count), 2), 256, 0, stream>>>(reinterpret_cast<const float2 *>(d_hop), reinterpret_cast<const float2 *>(d_hop0), g->d_work, nd));
-			if ((rc = tsdrgpu_fft_batch_internal(ctx, stream, g->d_work, (long long) nd, g->d_dd, (long long) nd, NULL, nd, 2, 0))) return rc;
-			D = g->d_dd;
-			d0 = reinterpret_cast<const float4 *>(g->d_dd + nd);
+			KL(ctx, "sbm_abs_diff", stream, sbm_abs_diff2<<<dim3(grid_for(nd, ctx->sm_count), 2), 256, 0, stream>>>(reinterpret_cast<const float2 *>(d_hop), reinterpret_cast<const float2 *>(d_hop0), g->d_work.ptr, nd));
+			if ((rc = tsdrgpu_fft_batch_internal(ctx, stream, g->d_work.ptr, (long long) nd, g->d_dd.ptr, (long long) nd, NULL, nd, 2, 0))) return rc;
+			D = g->d_dd.ptr;
+			d0 = reinterpret_cast<const float4 *>(g->d_dd.ptr + nd);
 		} else {                                              // pull it from rank 0 once its spectra are in place
-			KL(ctx, "sbm_abs_diff", stream, sbm_abs_diff<<<grid_for(nd, ctx->sm_count), 256, 0, stream>>>(reinterpret_cast<const float2 *>(d_hop), g->d_work, nd));
-			if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work, D, nd, 0))) return rc;
+			KL(ctx, "sbm_abs_diff", stream, sbm_abs_diff<<<grid_for(nd, ctx->sm_count), 256, 0, stream>>>(reinterpret_cast<const float2 *>(d_hop), g->d_work.ptr, nd));
+			if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work.ptr, D, nd, 0))) return rc;
 			KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_SPEC, epoch, all, all, (const int *) NULL, g->timeout_cycles));
 			d0 = reinterpret_cast<const float4 *>(g->peers.win[0] + g->off_d);
 		}
-		KL(ctx, "sbm_xcorr_pull", stream, sbm_xcorr_pull<<<grid_for(nd / 2, ctx->sm_count), 256, 0, stream>>>(d0, reinterpret_cast<const float4 *>(D), reinterpret_cast<float4 *>(g->d_p), nd / 2));
-		if ((rc = tsdrgpu_fft_internal(ctx, stream, g->d_p, nd, 1))) return rc;
-		if ((rc = tsdrgpu_argmax_mag_internal(ctx, stream, g->d_p, nd, g->d_part, g->d_lag))) return rc;
+		KL(ctx, "sbm_xcorr_pull", stream, sbm_xcorr_pull<<<grid_for(nd / 2, ctx->sm_count), 256, 0, stream>>>(d0, reinterpret_cast<const float4 *>(D), reinterpret_cast<float4 *>(g->d_p.ptr), nd / 2));
+		if ((rc = tsdrgpu_fft_internal(ctx, stream, g->d_p.ptr, nd, 1))) return rc;
+		if ((rc = tsdrgpu_argmax_mag_internal(ctx, stream, g->d_p.ptr, nd, g->d_part.ptr, g->d_lag.ptr))) return rc;
 	} else if (!d_hop0) {                                     // rank 0 serves its difference spectrum; its own lag stays 0
-		KL(ctx, "sbm_abs_diff", stream, sbm_abs_diff<<<grid_for(nd, ctx->sm_count), 256, 0, stream>>>(reinterpret_cast<const float2 *>(d_hop), g->d_work, nd));
-		if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work, D, nd, 0))) return rc;
+		KL(ctx, "sbm_abs_diff", stream, sbm_abs_diff<<<grid_for(nd, ctx->sm_count), 256, 0, stream>>>(reinterpret_cast<const float2 *>(d_hop), g->d_work.ptr, nd));
+		if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work.ptr, D, nd, 0))) return rc;
 		KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_SPEC, epoch, all, all, (const int *) NULL, g->timeout_cycles));
 	}
 	if (forked) CU_TRY(ctx, cudaStreamWaitEvent(stream, g->ev_join, 0));
-	KL(ctx, "sbm_permute_ramp", stream, sbm_permute_ramp<<<grid_for(N, ctx->sm_count, 16), 256, 0, stream>>>(g->d_x, Xp, N, g->log2H, g->d_lag));
-	KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_LAG, epoch, all, all, g->d_lag, g->timeout_cycles));
+	KL(ctx, "sbm_permute_ramp", stream, sbm_permute_ramp<<<grid_for(N, ctx->sm_count, 16), 256, 0, stream>>>(g->d_x.ptr, Xp, N, g->log2H, g->d_lag.ptr));
+	KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_LAG, epoch, all, all, g->d_lag.ptr, g->timeout_cycles));
 	// ---- phase 2: all-to-all #1 (pull this rank's run from everybody), the block transform with the reference's stage angles
 	{
 		PullArgs A; A.peers = g->peers; A.off_xp = g->off_x; A.H = H; A.rank = rank; A.per = N / (unsigned) H;
-		KL(ctx, "sbm_pull_blocks", stream, sbm_pull_blocks<<<grid_for(N / 2, ctx->sm_count, 16), 256, 0, stream>>>(A, reinterpret_cast<float4 *>(g->d_work)));
+		KL(ctx, "sbm_pull_blocks", stream, sbm_pull_blocks<<<grid_for(N / 2, ctx->sm_count, 16), 256, 0, stream>>>(A, reinterpret_cast<float4 *>(g->d_work.ptr)));
 	}
-	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work, Ablk, N, 1))) return rc;
+	if ((rc = tsdrgpu_fft_oop_internal(ctx, stream, g->d_work.ptr, Ablk, N, 1))) return rc;
 	KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_MIX, epoch, all, all, (const int *) NULL, g->timeout_cycles));
 	// ---- phase 3: all-to-all #2 + the reference's last log2 H stages + |.| pushed into the root's (time-contiguous) stream
 	{
@@ -450,7 +460,7 @@ int tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stream_, const fl
 	KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_RES, epoch, 1u << g->root, rank == g->root ? all : 0u, (const int *) NULL, g->timeout_cycles));
 	// ---- phase 4 (root): the stream is complete and time-contiguous in the window; hand it to the caller
 	// (d_stream_out == NULL: the caller reads it in place, tsdrgpu_superb_mgpu_stream_window -- on this stream, before its next stitch)
-	if (rank == g->root && d_stream_out) CU_TRY(ctx, cudaMemcpyAsync(d_stream_out, g->win + g->off_r, sizeof(float) * (size_t) H * N, cudaMemcpyDeviceToDevice, stream));
+	if (rank == g->root && d_stream_out) CU_TRY(ctx, cudaMemcpyAsync(d_stream_out, g->win.ptr + g->off_r, sizeof(float) * (size_t) H * N, cudaMemcpyDeviceToDevice, stream));
 	if (h_n) *h_n = N;
 	return TSDRGPU_OK;
 }
@@ -460,7 +470,7 @@ int tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stream_, const fl
 // overwrites it (the peers cannot get there earlier: they wait for the root's flags of the next stitch).
 int tsdrgpu_superb_mgpu_stream_window(tsdrgpu_superb_mgpu_t *g, float **d_stream) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, g != NULL && d_stream != NULL);
-	*d_stream = reinterpret_cast<float *>(g->win + g->off_r);
+	*d_stream = reinterpret_cast<float *>(g->win.ptr + g->off_r);
 	return TSDRGPU_OK;
 }
 
@@ -471,7 +481,7 @@ int tsdrgpu_superb_mgpu_lags(tsdrgpu_superb_mgpu_t *g, void *stream_, int *h_lag
 	BIND(ctx);
 	cudaStream_t stream = (cudaStream_t) stream_;
 	WinHeader h;
-	CU_TRY(ctx, cudaMemcpyAsync(&h, g->win, sizeof h, cudaMemcpyDeviceToHost, stream));
+	CU_TRY(ctx, cudaMemcpyAsync(&h, g->win.ptr, sizeof h, cudaMemcpyDeviceToHost, stream));
 	CU_TRY(ctx, cudaStreamSynchronize(stream));
 	if (h_lags) for (int q = 0; q < g->H; q++) h_lags[q] = h.lag[q];
 	if (h_status) *h_status = h.status;
