@@ -355,18 +355,41 @@ __global__ void __launch_bounds__(256) fs_timelowpass(const float *__restrict__ 
 	}
 }
 
+// the normalised pixel v (dsp.c:72-79).  The quotient is formed for markers too and then dropped: without a branch around the
+// division, the compiler keeps the divisor's reciprocal across unrolled pixels and their loads in flight together.
+__device__ __forceinline__ float norm_px(float x, float lastmin, float span) {
+	const float q = __fdiv_rn(__fsub_rn(x, lastmin), span);
+	return px_is_marker(x) ? x : q;
+}
+__device__ __forceinline__ bool finite_px(float s) { return (__float_as_uint(s) & 0x7f800000u) != 0x7f800000u; }
+// the values of v for which a motion blur of 0 does not pass v through unchanged (fs_collapse_tiles<true>): NaN, +-inf, -0.0f
+__device__ __forceinline__ unsigned norm_px_bad(float v) { return !finite_px(v) | (__float_as_uint(v) == 0x80000000u); }
+
 // auto-gain pass 2 fused with the temporal IIR (default stage order): out[f][i] = screen_f[i] where
 // screen_f = lowpass(screen_{f-1}, normalise_f(in[f][i])).  Saves one write + one read of the normalised frames.
-template <bool VEC>
+// REDO: after the collapse that normalised on load (motion blur 0, fs_collapse_tiles<true> / fs_collapse<true>), `out` already holds
+// v.  A thread whose start-of-batch screen values are finite, in a batch whose certificate word is clear, then only carries the
+// last frame into the screen (out[F-1] == screen_F); every other thread runs the literal update for its pixels, and one whose
+// screen was not finite sets the word, so that the gated collapse after this kernel redoes the sums from `out`.
+template <bool VEC, bool REDO>
 __global__ void __launch_bounds__(256) fs_norm_lowpass(const float *__restrict__ in, float *out, float *screen, size_t n, int nframes,
-                                                       const FrameParams *__restrict__ params, float coeff, double fresh) {
+                                                       const FrameParams *__restrict__ params, float coeff, double fresh, unsigned *cert) {
 	extern __shared__ float2 s_par[];                    // (lastmin, span) per frame
 	for (int f = threadIdx.x; f < nframes; f += blockDim.x) s_par[f] = make_float2(params[f].lastmin, params[f].span);
 	__syncthreads();
+	const bool redo_all = REDO && *cert != 0;
+	int set = 0;                                         // REDO: a screen value was not finite
 	if (VEC) {                                           // 4 pixels per thread, 16-byte loads and stores (n % 4 == 0, aligned bases: checked by the host)
 		const size_t n4 = n >> 2;
 		for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t) gridDim.x * blockDim.x) {
 			float4 sc = reinterpret_cast<float4 *>(screen)[i];
+			if (REDO && !redo_all) {
+				if (finite_px(sc.x) && finite_px(sc.y) && finite_px(sc.z) && finite_px(sc.w)) {
+					reinterpret_cast<float4 *>(screen)[i] = reinterpret_cast<const float4 *>(out + (size_t) (nframes - 1) * n)[i];
+					continue;
+				}
+				set = 1;
+			}
 			float s4[4] = {sc.x, sc.y, sc.z, sc.w};
 			for (int f0 = 0; f0 < nframes; f0 += 4) {         // 4 frames of loads in flight, then the ordered updates
 				float4 q4[4];
@@ -380,7 +403,7 @@ __global__ void __launch_bounds__(256) fs_norm_lowpass(const float *__restrict__
 					const float2 p = s_par[f];
 					#pragma unroll
 					for (int u = 0; u < 4; u++) {
-						const float v = px_is_marker(raw[u]) ? raw[u] : __fdiv_rn(__fsub_rn(raw[u], p.x), p.y);
+						const float v = norm_px(raw[u], p.x, p.y);
 						const float old = __fmul_rn(s4[u], coeff);
 						s4[u] = __double2float_rn(__dadd_rn((double) old, __dmul_rn((double) v, fresh)));
 					}
@@ -389,30 +412,35 @@ __global__ void __launch_bounds__(256) fs_norm_lowpass(const float *__restrict__
 			}
 			reinterpret_cast<float4 *>(screen)[i] = make_float4(s4[0], s4[1], s4[2], s4[3]);
 		}
-		return;
-	}
-	// frames of an odd number of pixels (1481 x 1125, 507 x 525) start at every alignment: one pixel per thread, and because a
-	// thread then has only 4 bytes per frame to ask for, SIXTEEN frames of loads are in flight before the ordered updates run
-	// (with four the kernel falls far behind the 16-byte path in the share of the HBM roofline it reaches)
-	for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
-		float s = screen[i];
-		for (int f0 = 0; f0 < nframes; f0 += 16) {
-			float raw[16];
-			#pragma unroll
-			for (int g = 0; g < 16; g++) if (f0 + g < nframes) raw[g] = ldg_stream_f1(in + (size_t) (f0 + g) * n + i);
-			#pragma unroll
-			for (int g = 0; g < 16; g++) {
-				const int f = f0 + g;
-				if (f >= nframes) break;
-				const float2 p = s_par[f];
-				const float v = px_is_marker(raw[g]) ? raw[g] : __fdiv_rn(__fsub_rn(raw[g], p.x), p.y);
-				const float old = __fmul_rn(s, coeff);
-				s = __double2float_rn(__dadd_rn((double) old, __dmul_rn((double) v, fresh)));
-				out[(size_t) f * n + i] = s;
+	} else {
+		// frames of an odd number of pixels (1481 x 1125, 507 x 525) start at every alignment: one pixel per thread, and because a
+		// thread then has only 4 bytes per frame to ask for, SIXTEEN frames of loads are in flight before the ordered updates run
+		// (with four the kernel falls far behind the 16-byte path in the share of the HBM roofline it reaches)
+		for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
+			float s = screen[i];
+			if (REDO && !redo_all) {
+				if (finite_px(s)) { screen[i] = out[(size_t) (nframes - 1) * n + i]; continue; }
+				set = 1;
 			}
+			for (int f0 = 0; f0 < nframes; f0 += 16) {
+				float raw[16];
+				#pragma unroll
+				for (int g = 0; g < 16; g++) if (f0 + g < nframes) raw[g] = ldg_stream_f1(in + (size_t) (f0 + g) * n + i);
+				#pragma unroll
+				for (int g = 0; g < 16; g++) {
+					const int f = f0 + g;
+					if (f >= nframes) break;
+					const float2 p = s_par[f];
+					const float v = norm_px(raw[g], p.x, p.y);
+					const float old = __fmul_rn(s, coeff);
+					s = __double2float_rn(__dadd_rn((double) old, __dmul_rn((double) v, fresh)));
+					out[(size_t) f * n + i] = s;
+				}
+			}
+			screen[i] = s;
 		}
-		screen[i] = s;
 	}
+	if (REDO && __syncthreads_or(set) && threadIdx.x == 0) atomicOr(cert, 1u);
 }
 
 // ---------------------------------------------------------------- row / column collapse (dsp.c:96-110)
@@ -455,19 +483,48 @@ __device__ __forceinline__ void tma_box3(unsigned dst_smem, const CUtensorMap *m
 	             :: "r"(dst_smem), "l"(reinterpret_cast<unsigned long long>(map)), "r"(x), "r"(y), "r"(z), "r"(bar) : "memory");
 }
 
-__global__ void __launch_bounds__(CT_THREADS) fs_collapse_tiles(const __grid_constant__ CUtensorMap cmap, const __grid_constant__ CUtensorMap rmap,
-                                                                int w, int h, float *__restrict__ wbuf, float *__restrict__ hbuf, int col_ctas) {
+__device__ __forceinline__ void tma_store_box3(const CUtensorMap *map, int x, int y, int z, unsigned src_smem) {
+	asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];"
+	             :: "l"(reinterpret_cast<unsigned long long>(map)), "r"(x), "r"(y), "r"(z), "r"(src_smem) : "memory");
+	asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+template <int N> __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
+
+// ---- normalise on load (default stage order, motion blur 0)
+// With motion blur c = 0 the temporal IIR is the identity: fs_norm_lowpass forms s' = (double) (s * c) + (double) v rounded to
+// float, and s * c is a signed zero for every finite screen value s, so s' == v bit for bit unless v is NaN, +-inf or -0.0f
+// (+0.0f + -0.0f is +0.0f).  The collapse then normalises the raw pixels as it loads them, sums v, and its column CTAs (which see
+// every pixel once) write v as the low-passed frames and set the batch's certificate word when any v of the batch is one of those
+// values.  fs_norm_lowpass<REDO> and the gated collapse after it redo the batch literally when the word is set.
+
+// NORM = false: the literal collapse of `cmap`/`rmap` (one warp per CTA); with `gate`, only when *gate is set.
+// NORM = true: the collapse of the raw frames normalised on load (CT_NTHREADS per CTA).  All warps normalise each landed box in
+// place (the division makes that issue-bound for one warp), then warp 0's owner lanes sum it as above; a column CTA stores
+// its normalised box through `smap` (the low-passed frames) and checks it for the certificate.  A slot is refilled two stages
+// after its store was issued, once the store has read it.
+constexpr int CT_NTHREADS = 128;
+template <bool NORM>
+__global__ void __launch_bounds__(NORM ? CT_NTHREADS : CT_THREADS) fs_collapse_tiles(const __grid_constant__ CUtensorMap cmap, const __grid_constant__ CUtensorMap rmap,
+                                                                                     const __grid_constant__ CUtensorMap smap, int w, int h,
+                                                                                     float *__restrict__ wbuf, float *__restrict__ hbuf, int col_ctas,
+                                                                                     const unsigned *gate, const FrameParams *__restrict__ params,
+                                                                                     unsigned *cert) {
+	if (!NORM && gate && *gate == 0) return;             // the batch's normalise-on-load pass was exact
 	extern __shared__ unsigned char ct_smem[];
 	__shared__ __align__(8) unsigned long long bars[CT_CSTAGES > CT_RSTAGES ? CT_CSTAGES : CT_RSTAGES];
 	const unsigned raw = (unsigned) __cvta_generic_to_shared(ct_smem), ring_a = (raw + 1023u) & ~1023u;
-	const float *ring = reinterpret_cast<const float *>(ct_smem + (ring_a - raw));
+	float *ring = reinterpret_cast<float *>(ct_smem + (ring_a - raw));
 	const unsigned bar_a = (unsigned) __cvta_generic_to_shared(bars);
 	const int f = blockIdx.y, tid = threadIdx.x;
 	const bool colcta = (int) blockIdx.x < col_ctas;
+	const bool store = NORM && colcta;
 	const int stages = colcta ? CT_CSTAGES : CT_RSTAGES;
+	const int lead = store ? stages - 2 : stages - 1;    // boxes in flight ahead of the one being summed
 	const unsigned box_bytes = colcta ? CT_COLS * CT_CROWS * 4 : CT_RCOLS * CT_ROWS * 4;
 	const int x0 = colcta ? blockIdx.x * CT_COLS : 0, y0 = colcta ? 0 : ((int) blockIdx.x - col_ctas) * CT_ROWS;
 	const int nit = colcta ? (h + CT_CROWS - 1) / CT_CROWS : (w + CT_RCOLS - 1) / CT_RCOLS;
+	float lastmin = 0.0f, span = 1.0f;
+	if (NORM) { lastmin = params[f].lastmin; span = params[f].span; }
 	if (tid == 0) {
 		for (int st = 0; st < stages; st++) mbar_init(bar_a + 8 * st, 1);
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -481,14 +538,46 @@ __global__ void __launch_bounds__(CT_THREADS) fs_collapse_tiles(const __grid_con
 		if (colcta) tma_box3(ring_a + slot * box_bytes, &cmap, x0, it * CT_CROWS, f, bar);
 		else tma_box3(ring_a + slot * box_bytes, &rmap, it * CT_RCOLS, y0, f, bar);
 	};
-	if (tid == 0) for (int st = 0; st < stages - 1; st++) issue(st);
+	if (tid == 0) for (int st = 0; st < lead; st++) issue(st);
 	float acc = 0.0f;
-	const bool owner = colcta ? (tid < w - x0) : (tid < h - y0);        // one thread per column / row of the CTA
+	unsigned bad = 0;
+	// one thread of warp 0 per column / row of the CTA
+	const bool owner = tid < CT_COLS && (colcta ? (tid < w - x0) : (tid < h - y0));
 	for (int it = 0; it < nit; it++) {
 		__syncthreads();                                 // everybody is done with the slot of stage it-1: it may be refilled
-		if (tid == 0) issue(it + stages - 1);
+		if (tid == 0) {
+			if (store) tma_store_wait_read<1>();         // the store of stage it-2 has read the slot about to be refilled
+			issue(it + lead);
+		}
 		const int slot = it % stages;
 		mbar_wait(bar_a + 8 * slot, (unsigned) ((it / stages) & 1));
+		if (NORM) {
+			float *box = ring + slot * (box_bytes / 4);
+			if (store) {
+				constexpr int K = CT_COLS * CT_CROWS / CT_NTHREADS;
+				const int rows = min(CT_CROWS, h - it * CT_CROWS), cols = min(CT_COLS, w - x0);
+				float x[K];
+				#pragma unroll
+				for (int k = 0; k < K; k++) x[k] = box[tid + k * CT_NTHREADS];
+				#pragma unroll
+				for (int k = 0; k < K; k++) {
+					const int e = tid + k * CT_NTHREADS;
+					const float v = norm_px(x[k], lastmin, span);
+					box[e] = v;
+					if (e / CT_COLS < rows && e % CT_COLS < cols) bad |= norm_px_bad(v);      // pixels of the frame only
+				}
+			} else {                                     // the swizzle permutes a row's chunks: in place it does not matter
+				constexpr int K = CT_RCOLS * CT_ROWS / CT_NTHREADS;
+				float x[K];
+				#pragma unroll
+				for (int k = 0; k < K; k++) x[k] = box[tid + k * CT_NTHREADS];
+				#pragma unroll
+				for (int k = 0; k < K; k++) box[tid + k * CT_NTHREADS] = norm_px(x[k], lastmin, span);
+			}
+			asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // the box's generic writes before the bulk copies' access
+			__syncthreads();
+			if (store && tid == 0) tma_store_box3(&smap, x0, it * CT_CROWS, f, ring_a + slot * box_bytes);   // clipped to the frame
+		}
 		if (!owner) continue;
 		if (colcta) {
 			const float *buf = ring + slot * (CT_COLS * CT_CROWS) + tid;
@@ -515,6 +604,10 @@ __global__ void __launch_bounds__(CT_THREADS) fs_collapse_tiles(const __grid_con
 		}
 	}
 	if (owner) { if (colcta) wbuf[(size_t) f * w + x0 + tid] = acc; else hbuf[(size_t) f * h + y0 + tid] = acc; }
+	if (store) {                                         // uniform over the CTA
+		if (__syncthreads_or(bad) && tid == 0) atomicOr(cert, 1u);
+		if (tid == 0) tma_store_wait_read<0>();          // the ring stays until the last store has read it
+	}
 }
 
 // Rows at any alignment (odd widths: 1481, 507): every pixel copied with a 4-byte cp.async through a 4-stage ring.
@@ -523,11 +616,18 @@ __global__ void __launch_bounds__(CT_THREADS) fs_collapse_tiles(const __grid_con
 constexpr int CL_COLS = 128, CL_CROWS = 16, CL_ROWS = 32, CL_RCOLS = 64, CL_STAGES = 4;
 constexpr int CL_RPITCH = CL_RCOLS + 1;
 constexpr int CL_SMEM_FLOATS = CL_STAGES * (CL_CROWS * CL_COLS > CL_ROWS * CL_RPITCH ? CL_CROWS * CL_COLS : CL_ROWS * CL_RPITCH);
+// NORM and `gate` as fs_collapse_tiles: with NORM every thread normalises the pixels it copied once they have landed, in place, and
+// in column CTAs also writes them to the low-passed frames `t2` and checks them for the certificate.
+template <bool NORM>
 __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in, int w, int h, float *__restrict__ wbuf,
-                                                   float *__restrict__ hbuf, int col_ctas) {
+                                                   float *__restrict__ hbuf, int col_ctas, const unsigned *gate,
+                                                   const FrameParams *__restrict__ params, float *__restrict__ t2, unsigned *cert) {
+	if (!NORM && gate && *gate == 0) return;             // the batch's normalise-on-load pass was exact
 	__shared__ __align__(16) float ring[CL_SMEM_FLOATS];
 	const int f = blockIdx.y, tid = threadIdx.x;
 	const float *src = in + (size_t) f * w * h;
+	float lastmin = 0.0f, span = 1.0f;
+	if (NORM) { lastmin = params[f].lastmin; span = params[f].span; }
 	if ((int) blockIdx.x < col_ctas) {
 		const int x0 = blockIdx.x * CL_COLS, cols = min(CL_COLS, w - x0);
 		const int nit = (h + CL_CROWS - 1) / CL_CROWS;
@@ -545,8 +645,22 @@ __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in,
 		};
 		for (int st = 0; st < CL_STAGES - 1; st++) issue(st);
 		float acc = 0.0f;
+		unsigned bad = 0;
 		for (int it = 0; it < nit; it++) {
 			__pipeline_wait_prior(CL_STAGES - 2);
+			if (NORM) {                                  // this thread's copies of stage `it` have landed
+				float *dst = ring + (it % CL_STAGES) * (CL_CROWS * CL_COLS);
+				const int y0 = it * CL_CROWS, rows = min(CL_CROWS, h - y0);
+				float *t0 = t2 + (size_t) f * w * h + (size_t) y0 * w + x0;
+				for (int idx = tid; idx < rows * CL_COLS; idx += 256) {
+					const int r = idx / CL_COLS, c = idx % CL_COLS;
+					if (c < cols) {
+						const float v = norm_px(dst[idx], lastmin, span);
+						dst[idx] = v; t0[r * w + c] = v;
+						bad |= norm_px_bad(v);
+					}
+				}
+			}
 			__syncthreads();                             // stage `it` has landed; the buffer of stage it-1 is free again
 			issue(it + CL_STAGES - 1);
 			if (tid < cols) {
@@ -559,6 +673,7 @@ __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in,
 			}
 		}
 		if (tid < cols) wbuf[(size_t) f * w + x0 + tid] = acc;
+		if (NORM && __syncthreads_or(bad) && tid == 0) atomicOr(cert, 1u);
 		return;
 	}
 	const int y0 = ((int) blockIdx.x - col_ctas) * CL_ROWS, rows = min(CL_ROWS, h - y0);
@@ -579,6 +694,14 @@ __global__ void __launch_bounds__(256) fs_collapse(const float *__restrict__ in,
 	float acc = 0.0f;
 	for (int it = 0; it < nit; it++) {
 		__pipeline_wait_prior(CL_STAGES - 2);
+		if (NORM) {
+			float *dst = ring + (it % CL_STAGES) * (CL_ROWS * CL_RPITCH);
+			const int cols = min(CL_RCOLS, w - it * CL_RCOLS);
+			for (int idx = tid; idx < rows * CL_RCOLS; idx += 256) {
+				const int r = idx / CL_RCOLS, c = idx % CL_RCOLS;
+				if (c < cols) dst[r * CL_RPITCH + c] = norm_px(dst[r * CL_RPITCH + c], lastmin, span);
+			}
+		}
 		__syncthreads();
 		issue(it + CL_STAGES - 1);
 		if (tid < rows) {
@@ -1122,7 +1245,8 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 
 // refresh the auto-gain fields of already written results (auto-gain-after-processing order)
 __global__ void fs_results_autogain(int nframes, const FrameParams *__restrict__ params, const SyncState *__restrict__ state,
-                                    tsdrgpu_frame_result_t *results) {
+                                    tsdrgpu_frame_result_t *results, unsigned *clear = NULL) {
+	if (clear && threadIdx.x == 0) *clear = 0;           // the certificate word of the batch about to be collapsed
 	for (int f = threadIdx.x; f < nframes; f += blockDim.x) {
 		if (params) { results[f].lastmax = params[f].lastmax; results[f].lastmin = params[f].lastmin; results[f].snr = params[f].snr; }
 		else { results[f].lastmax = state->lastmax; results[f].lastmin = state->lastmin; results[f].snr = state->snr; }
@@ -1304,28 +1428,50 @@ int encode_collapse_maps(tsdrgpu_ctx_t *ctx, const float *ptr, int w, int h, int
 	return TSDRGPU_OK;
 }
 
-// row and column sums of `nframes` frames: the tensor-map kernel on 16-byte rows, the cp.async kernel otherwise
+// the collapse that normalises the raw frames on load (fs_collapse_tiles<true> / fs_collapse<true>)
+struct NormOnLoad {
+	const FrameParams *params;                   // (lastmin, span) per frame
+	float *out;                                  // the normalised frames (aligned: a tensor map over it on the tiles path)
+	unsigned *cert;                              // certificate word, set when the batch has to be redone
+};
+
+// row and column sums of `nframes` frames: the tensor-map kernel on 16-byte rows, the cp.async kernel otherwise.
+// `name` labels the launch in the profile; with `gate`, the kernel returns at once unless *gate is set; with `norm`, src holds the
+// raw frames and the collapse normalises them on load.
 int launch_collapse(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *src, int w, int h, int nframes, float *wbuf, float *hbuf,
-                    CollapseMaps *cache, int ncache) {
+                    CollapseMaps *cache, int ncache, const char *name = "fs_collapse", const unsigned *gate = NULL,
+                    const NormOnLoad *norm = NULL) {
 	if ((w % 4 == 0) && ((reinterpret_cast<unsigned long long>(src) & 15ull) == 0)) {
-		CollapseMaps local, *m = NULL;
-		for (int i = 0; i < ncache && !m; i++)
-			if (cache[i].ptr == src && cache[i].w == w && cache[i].h == h && cache[i].nframes == nframes) m = &cache[i];
-		if (!m) {
-			m = &local;
+		auto maps = [&](const float *ptr, CollapseMaps *out) -> int {      // the maps over `ptr`, from the cache or encoded into it
+			for (int i = 0; i < ncache; i++)
+				if (cache[i].ptr == ptr && cache[i].w == w && cache[i].h == h && cache[i].nframes == nframes) { *out = cache[i]; return TSDRGPU_OK; }
+			int rc = encode_collapse_maps(ctx, ptr, w, h, nframes, out);
+			if (rc) return rc;
 			if (ncache) {                                // the frame stage collapses a handful of buffers: evict the oldest
 				for (int i = ncache - 1; i > 0; i--) cache[i] = cache[i - 1];
-				m = &cache[0];
+				cache[0] = *out;
 			}
-			int rc = encode_collapse_maps(ctx, src, w, h, nframes, m);
-			if (rc) { m->ptr = NULL; return rc; }
-		}
+			return TSDRGPU_OK;
+		};
+		CollapseMaps m, mo;
+		int rc;
+		if ((rc = maps(src, &m))) return rc;
+		if (norm && (rc = maps(norm->out, &mo))) return rc;
 		const int col_ctas = (w + CT_COLS - 1) / CT_COLS, row_ctas = (h + CT_ROWS - 1) / CT_ROWS;
-		CU_TRY(ctx, cudaFuncSetAttribute(fs_collapse_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
-		KL(ctx, "fs_collapse", stream, fs_collapse_tiles<<<dim3(col_ctas + row_ctas, nframes), CT_THREADS, CT_SMEM, stream>>>(m->col, m->row, w, h, wbuf, hbuf, col_ctas));
+		const dim3 grid(col_ctas + row_ctas, nframes);
+		if (norm) {
+			CU_TRY(ctx, cudaFuncSetAttribute(fs_collapse_tiles<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
+			KL(ctx, name, stream, fs_collapse_tiles<true><<<grid, CT_NTHREADS, CT_SMEM, stream>>>(m.col, m.row, mo.col, w, h, wbuf, hbuf, col_ctas, NULL,
+			                                                                                        norm->params, norm->cert));
+		} else {
+			CU_TRY(ctx, cudaFuncSetAttribute(fs_collapse_tiles<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
+			KL(ctx, name, stream, fs_collapse_tiles<false><<<grid, CT_THREADS, CT_SMEM, stream>>>(m.col, m.row, m.col, w, h, wbuf, hbuf, col_ctas, gate, NULL, NULL));
+		}
 	} else {
 		const int col_ctas = (w + CL_COLS - 1) / CL_COLS, row_ctas = (h + CL_ROWS - 1) / CL_ROWS;
-		KL(ctx, "fs_collapse", stream, fs_collapse<<<dim3(col_ctas + row_ctas, nframes), 256, 0, stream>>>(src, w, h, wbuf, hbuf, col_ctas));
+		const dim3 grid(col_ctas + row_ctas, nframes);
+		if (norm) KL(ctx, name, stream, fs_collapse<true><<<grid, 256, 0, stream>>>(src, w, h, wbuf, hbuf, col_ctas, NULL, norm->params, norm->out, norm->cert));
+		else KL(ctx, name, stream, fs_collapse<false><<<grid, 256, 0, stream>>>(src, w, h, wbuf, hbuf, col_ctas, gate, NULL, NULL, NULL));
 	}
 	return TSDRGPU_OK;
 }
@@ -1363,7 +1509,8 @@ struct tsdrgpu_framestage {
 	cudaStream_t s_side;
 	cudaEvent_t ev_ready[2];                     // main: collapse of this phase done -> side may start
 	cudaEvent_t ev_done[2];                      // side: sync + emit of this phase done -> buffers of the phase are free
-	CollapseMaps collapse_maps[4];               // fs_collapse_tiles' tensor maps of the buffers collapsed last (d_t2[0/1], d_t1)
+	CollapseMaps collapse_maps[6];               // fs_collapse_tiles' tensor maps of the buffers collapsed last (d_t2[0/1], d_t1, inputs)
+	DeviceBuf<unsigned> d_cert;                  // the batch's normalise-on-load certificate (fs_collapse_tiles<true>), cleared per batch
 };
 
 // hands a's buffer to b and b's to a (DeviceBuf can be neither copied nor moved)
@@ -1469,6 +1616,7 @@ static int create_handles(tsdrgpu_framestage *fs) {
 	CU_TRY(ctx, fs->d_chain.assign(10 * FS_MAX_STRIP));
 	CU_TRY(ctx, fs->d_resume.assign(64));
 	CU_TRY(ctx, cudaMemset(fs->d_resume.ptr, 0, 256));
+	CU_TRY(ctx, fs->d_cert.assign(1));
 	{   // highest priority: its single CTA should be placed as soon as an SM has room, ahead of the main stream's queued CTAs
 		int lo = 0, hi = 0;
 		CU_TRY(ctx, cudaDeviceGetStreamPriorityRange(&lo, &hi));
@@ -1620,8 +1768,8 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 	const size_t total = (size_t) nframes * n;
 
 	// collapse on `stream`, then sync search on `s2` (== stream unless overlapped)
-	auto collapse_sync = [&](const float *src, cudaStream_t s2) -> int {
-		if ((rc = launch_collapse(ctx, stream, src, w, h, nframes, fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, fs->collapse_maps, 4))) return rc;
+	auto collapse_sync = [&](const float *src, cudaStream_t s2, const char *name, const unsigned *gate) -> int {
+		if ((rc = launch_collapse(ctx, stream, src, w, h, nframes, fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, fs->collapse_maps, 6, name, gate))) return rc;
 		if (s2 != stream) {
 			CU_TRY(ctx, cudaEventRecord(fs->ev_ready[ph], stream));
 			CU_TRY(ctx, cudaStreamWaitEvent(s2, fs->ev_ready[ph], 0));
@@ -1664,19 +1812,31 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 		if (!aap) {
 			if ((rc = fs_autogain_batch(fs, stream, d_in, fuse ? NULL : fs->d_t1.ptr, nframes, n, lowpasscoeff, snr))) return rc;
 			lp_in = fs->d_t1.ptr;
-			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
+			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results,
+			                                                                                   fuse ? fs->d_cert.ptr : NULL));
 		}
+		// motion blur 0: the collapse normalises on load and writes T2 (fs_collapse_tiles<true>); then, gated by the batch's
+		// certificate, the literal low-pass from the start-of-batch screen (or, when clear, the screen's update from T2) and the
+		// literal collapse of T2
+		const bool norm_on_load = fuse && motionblur == 0.0f;
 		if (fuse) {
 			// one thread per four pixels on the 16-byte path, one per pixel otherwise (odd frame sizes, unaligned input)
 			const bool vec = ((n & 3) == 0) && (((reinterpret_cast<unsigned long long>(d_in) | reinterpret_cast<unsigned long long>(T2) | reinterpret_cast<unsigned long long>(fs->d_screen.ptr)) & 15ull) == 0);
 			const size_t threads = vec ? n / 4 : n;
 			const unsigned grid = (unsigned) ((threads + 255) / 256 ? (threads + 255) / 256 : 1);
-			if (vec) KL(ctx, "fs_norm_lowpass", stream, fs_norm_lowpass<true><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh));
-			else KL(ctx, "fs_norm_lowpass", stream, fs_norm_lowpass<false><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh));
+			const char *name = norm_on_load ? "fs_redo_lowpass" : "fs_norm_lowpass";
+			if (norm_on_load) {
+				const NormOnLoad norm = {fs->d_params.ptr, T2, fs->d_cert.ptr};
+				if ((rc = launch_collapse(ctx, stream, d_in, w, h, nframes, fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, fs->collapse_maps, 6,
+				                          "fs_collapse", NULL, &norm))) return rc;
+				if (vec) KL(ctx, name, stream, (fs_norm_lowpass<true, true><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh, fs->d_cert.ptr)));
+				else KL(ctx, name, stream, (fs_norm_lowpass<false, true><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh, fs->d_cert.ptr)));
+			} else if (vec) KL(ctx, name, stream, (fs_norm_lowpass<true, false><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh, NULL)));
+			else KL(ctx, name, stream, (fs_norm_lowpass<false, false><<<grid, 256, sizeof(float2) * nframes, stream>>>(d_in, T2, fs->d_screen.ptr, n, nframes, fs->d_params.ptr, motionblur, fresh, NULL)));
 		}
 		else KL(ctx, "fs_timelowpass", stream, fs_timelowpass<<<gx, 256, 0, stream>>>(lp_in, T2, fs->d_screen.ptr, n, nframes, motionblur, fresh));
 		if (overlapped) tail = fs->s_side;
-		if ((rc = collapse_sync(T2, tail))) return rc;
+		if ((rc = collapse_sync(T2, tail, norm_on_load ? "fs_redo_collapse" : "fs_collapse", norm_on_load ? fs->d_cert.ptr : NULL))) return rc;
 		float *dst = aap ? fs->d_t1.ptr : d_out;
 		if ((rc = emit(T2, dst, !superres, false, &res, tail))) return rc;
 		if (aap) {
@@ -1689,7 +1849,7 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 			if ((rc = fs_autogain_batch(fs, stream, d_in, fs->d_t1.ptr, nframes, n, lowpasscoeff, snr))) return rc;
 			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
 		} else if ((rc = fs_copy_async(ctx, stream, d_in, fs->d_t1.ptr, total))) return rc;
-		if ((rc = collapse_sync(work, stream))) return rc;
+		if ((rc = collapse_sync(work, stream, "fs_collapse", NULL))) return rc;
 		if ((rc = emit(work, T2, (motionblur == 0.0f) && !superres, true, &res, stream))) return rc;
 		float *lp_out = aap ? ((res == fs->d_t1.ptr) ? T2 : fs->d_t1.ptr) : d_out;
 		KL(ctx, "fs_timelowpass", stream, fs_timelowpass<<<gx, 256, 0, stream>>>(res, lp_out, fs->d_screen.ptr, n, nframes, motionblur, fresh));
