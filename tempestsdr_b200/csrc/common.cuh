@@ -4,11 +4,16 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <deque>
 #include <mutex>
 #include <vector>
 
 #include "../../include/tsdrgpu.h"
 #include "devbuf.h"
+
+// a twiddle table of the transforms (fft.cu): which one, and its device copy
+struct FftTableKey { int kind; long long a, b, c; double eps; };
+struct FftTable { FftTableKey key; DeviceBuf<float2> d; };
 
 struct tsdrgpu_ctx {
 	int device;
@@ -18,7 +23,10 @@ struct tsdrgpu_ctx {
 	// scratch owned by the context (grown on demand, reused across calls on the same stream)
 	DeviceBuf<unsigned char> scratch[4];
 	PinnedBuf<unsigned char> pinned;      // small pinned staging area for descriptor uploads / scalar read-backs
-	std::mutex mu;
+	std::mutex mu;                        // guards the profiling records and the FFT tables
+	// the transforms' twiddle tables, built on first use (a deque never moves them: DeviceBuf cannot move), and whether the
+	// pass kernels' shared-memory limit has been raised
+	std::deque<FftTable> fft_tables; bool fft_attrs_set = false;
 	// optional per-kernel timing (bench.py's roofline): CUDA events on the launching stream around named launches
 	bool profiling;
 	struct ProfRec { int id; cudaEvent_t a, b; };
@@ -105,6 +113,7 @@ int tsdrgpu_fft_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, 
 int tsdrgpu_fft_oop_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, unsigned long long n_pow2, int inverse);
 int tsdrgpu_fft_batch_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, long long in_bs, float2 *out, long long out_bs,
                                float2 *scratch, unsigned long long n_pow2, unsigned batch, int inverse);
+bool tsdrgpu_fft_true_dft();          // TSDRGPU_FFT_TRUE_DFT: the exact DFT's stage angles instead of the reference's
 int tsdrgpu_argmax_mag_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *x, unsigned n, void *d_part, int *d_result);
 int fs_copy_async(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, size_t total);
 // enhance.cu: NLM then CLAHE on delivered frames, modes and parameters as the frame stage's setters take them

@@ -23,7 +23,6 @@
 #include <math.h>
 #include <stdlib.h>
 #include <vector>
-#include <mutex>
 
 namespace {
 
@@ -652,64 +651,10 @@ inline unsigned grid1d(unsigned long long n, int sm_count) {
 	return (unsigned) (want < cap ? (want ? want : 1) : cap);
 }
 
-bool g_attr_set[64] = {false};      // per device: the pass kernels' dynamic shared-memory limit has been raised
-// per-pass layer-twiddle tables (see fft_pass_kernel), built on the host in double precision and cached
-struct StageTab { int device, log2L, l_base, pert; float2 *d; };
-std::vector<StageTab> g_stage_tabs;
-std::mutex g_tw_mu;
-
-int stage_table(tsdrgpu_ctx_t *ctx, int log2L, int l_base, const double *eps_all, const float2 **out) {
-	static const bool exact_dft = getenv("TSDRGPU_FFT_TRUE_DFT") != NULL;      // opt out: the mathematically exact DFT
-	double eps[FFT_MAX_LOG2L + 1];
-	int pert = 0;
-	for (int sidx = 0; sidx < log2L; sidx++) {
-		eps[sidx] = (!exact_dft && eps_all && l_base + sidx < 40) ? eps_all[l_base + sidx] : 0.0;
-		if (eps[sidx] != 0.0) pert = 1;
-	}
-	std::lock_guard<std::mutex> lock(g_tw_mu);
-	for (auto &t : g_stage_tabs) if (t.device == ctx->device && t.log2L == log2L && t.l_base == (pert ? l_base : -1) && t.pert == pert) { *out = t.d; return TSDRGPU_OK; }
-	const int L = 1 << log2L;
-	std::vector<float2> h((size_t) L);
-	for (int sidx = 0; sidx < log2L; sidx++) {
-		const int blk = 1 << sidx;
-		for (int K = 0; K < blk; K++) {
-			const double ang = -3.14159265358979323846 * ((double) K / (double) blk) * (1.0 + eps[sidx]);
-			h[(size_t) blk - 1 + K] = make_float2((float) cos(ang), (float) sin(ang));
-		}
-	}
-	h[(size_t) L - 1] = make_float2(1.0f, 0.0f);
-	StageTab t; t.device = ctx->device; t.log2L = log2L; t.l_base = pert ? l_base : -1; t.pert = pert;
-	CU_TRY(ctx, cudaMalloc(&t.d, sizeof(float2) * L));
-	CU_TRY(ctx, cudaMemcpy(t.d, h.data(), sizeof(float2) * L, cudaMemcpyHostToDevice));
-	g_stage_tabs.push_back(t);
-	*out = t.d;
-	return TSDRGPU_OK;
-}
-
-// W_M^(col * L8 * j) for every column of a pass and j = 0..7 (see fft_pass_kernel), built on the host, cached
-struct StepTab { int device; unsigned long long M; unsigned ncols, L8; float2 *d; };
-std::vector<StepTab> g_step_tabs;
-int step_table(tsdrgpu_ctx_t *ctx, unsigned long long M, unsigned ncols, unsigned L8, const float2 **out) {
-	std::lock_guard<std::mutex> lock(g_tw_mu);
-	for (auto &t : g_step_tabs) if (t.device == ctx->device && t.M == M && t.ncols == ncols && t.L8 == L8) { *out = t.d; return TSDRGPU_OK; }
-	std::vector<float2> h((size_t) ncols * 8);
-	for (unsigned col = 0; col < ncols; col++)
-		for (unsigned j = 0; j < 8; j++) {
-			const unsigned long long e = ((unsigned long long) col * (unsigned long long) (L8 * j)) & (M - 1);
-			const double ang = -2.0 * 3.14159265358979323846 * ((double) e / (double) M);
-			h[(size_t) col * 8 + j] = make_float2((float) cos(ang), (float) sin(ang));
-		}
-	StepTab t; t.device = ctx->device; t.M = M; t.ncols = ncols; t.L8 = L8;
-	CU_TRY(ctx, cudaMalloc(&t.d, sizeof(float2) * h.size()));
-	CU_TRY(ctx, cudaMemcpy(t.d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice));
-	g_step_tabs.push_back(t);
-	*out = t.d;
-	return TSDRGPU_OK;
-}
-
-int ensure_table(tsdrgpu_ctx_t *ctx, cudaStream_t stream) {
-	(void) stream;
-	if (g_attr_set[ctx->device]) return TSDRGPU_OK;
+// the pass kernels' dynamic shared-memory limit, raised once per context (ctx->mu held): before any of them is launched or has
+// its occupancy queried
+int pass_attrs(tsdrgpu_ctx_t *ctx) {
+	if (ctx->fft_attrs_set) return TSDRGPU_OK;
 	const int max_smem = (int) (2 * sizeof(float2) * FFT_MAX_ELEMS);     // ping-pong
 #define SET_ATTR(l) CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
 	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
@@ -718,8 +663,61 @@ int ensure_table(tsdrgpu_ctx_t *ctx, cudaStream_t stream) {
 	CU_TRY(ctx, cudaFuncSetAttribute(fft_acc_kernel<l>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem))
 	SET_ATTR(3); SET_ATTR(4); SET_ATTR(5); SET_ATTR(6); SET_ATTR(7); SET_ATTR(8); SET_ATTR(9); SET_ATTR(10); SET_ATTR(11);
 #undef SET_ATTR
-	g_attr_set[ctx->device] = true;
+	ctx->fft_attrs_set = true;
 	return TSDRGPU_OK;
+}
+
+// The context's twiddle table `key` (tsdrgpu_ctx::fft_tables), n entries computed on the host by fill(h) on first use.  The
+// first table also raises the pass kernels' shared-memory limit: every pass launch looks its stage table up first.
+enum { TAB_STAGE, TAB_STEP, TAB_LAST };
+template <class Fill> int fft_table(tsdrgpu_ctx_t *ctx, FftTableKey key, size_t n, Fill fill, const float2 **out) {
+	std::lock_guard<std::mutex> lock(ctx->mu);
+	for (auto &t : ctx->fft_tables)
+		if (t.key.kind == key.kind && t.key.a == key.a && t.key.b == key.b && t.key.c == key.c && t.key.eps == key.eps) { *out = t.d.ptr; return TSDRGPU_OK; }
+	if (const int rc = pass_attrs(ctx)) return rc;
+	std::vector<float2> h(n);
+	fill(h.data());
+	ctx->fft_tables.emplace_back();
+	FftTable &t = ctx->fft_tables.back();
+	t.key = key;
+	cudaError_t e = t.d.assign(n);
+	if (e == cudaSuccess) e = cudaMemcpy(t.d.ptr, h.data(), sizeof(float2) * n, cudaMemcpyHostToDevice);
+	if (e != cudaSuccess) { ctx->fft_tables.pop_back(); return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "FFT twiddle table", e, __FILE__, __LINE__); }
+	*out = t.d.ptr;
+	return TSDRGPU_OK;
+}
+
+// per-pass layer-twiddle tables (see fft_pass_kernel), built on the host in double precision
+int stage_table(tsdrgpu_ctx_t *ctx, int log2L, int l_base, const double *eps_all, const float2 **out) {
+	double eps[FFT_MAX_LOG2L + 1];
+	int pert = 0;
+	for (int sidx = 0; sidx < log2L; sidx++) {
+		eps[sidx] = (!tsdrgpu_fft_true_dft() && eps_all && l_base + sidx < 40) ? eps_all[l_base + sidx] : 0.0;
+		if (eps[sidx] != 0.0) pert = 1;
+	}
+	const int L = 1 << log2L;
+	return fft_table(ctx, {TAB_STAGE, log2L, pert ? l_base : -1, pert, 0.0}, (size_t) L, [&](float2 *h) {
+		for (int sidx = 0; sidx < log2L; sidx++) {
+			const int blk = 1 << sidx;
+			for (int K = 0; K < blk; K++) {
+				const double ang = -3.14159265358979323846 * ((double) K / (double) blk) * (1.0 + eps[sidx]);
+				h[(size_t) blk - 1 + K] = make_float2((float) cos(ang), (float) sin(ang));
+			}
+		}
+		h[(size_t) L - 1] = make_float2(1.0f, 0.0f);
+	}, out);
+}
+
+// W_M^(col * L8 * j) for every column of a pass and j = 0..7 (see fft_pass_kernel), built on the host
+int step_table(tsdrgpu_ctx_t *ctx, unsigned long long M, unsigned ncols, unsigned L8, const float2 **out) {
+	return fft_table(ctx, {TAB_STEP, (long long) M, ncols, L8, 0.0}, (size_t) ncols * 8, [&](float2 *h) {
+		for (unsigned col = 0; col < ncols; col++)
+			for (unsigned j = 0; j < 8; j++) {
+				const unsigned long long e = ((unsigned long long) col * (unsigned long long) (L8 * j)) & (M - 1);
+				const double ang = -2.0 * 3.14159265358979323846 * ((double) e / (double) M);
+				h[(size_t) col * 8 + j] = make_float2((float) cos(ang), (float) sin(ang));
+			}
+	}, out);
 }
 
 int bundle_for(int log2L, unsigned long long lines, bool contiguous_lines = false) {
@@ -881,10 +879,12 @@ unsigned ilog2(unsigned long long n) { unsigned m = 0; while ((n >>= 1) != 0) m+
 
 }  // namespace
 
+// opt out of the reference's stage angles: every transform is the mathematically exact DFT (read once per process)
+bool tsdrgpu_fft_true_dft() { static const bool on = getenv("TSDRGPU_FFT_TRUE_DFT") != NULL; return on; }
+
 // internal entry used by other translation units
 int tsdrgpu_fft_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, unsigned long long n_pow2, int inverse) {
-	int rc = ensure_table(ctx, stream);
-	if (rc) return rc;
+	int rc;
 	if (n_pow2 <= 1) return TSDRGPU_OK;
 	void *scratch;
 	if ((rc = tsdrgpu_scratch(ctx, 0, sizeof(float2) * n_pow2, &scratch))) return rc;
@@ -894,8 +894,7 @@ int tsdrgpu_fft_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, 
 
 // out of place: out = FFT(in), both n_pow2 complex, `in` untouched
 int tsdrgpu_fft_oop_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, unsigned long long n_pow2, int inverse) {
-	int rc = ensure_table(ctx, stream);
-	if (rc) return rc;
+	int rc;
 	if (n_pow2 <= 1) { if (n_pow2 == 1) CU_TRY(ctx, cudaMemcpyAsync(out, in, sizeof(float2), cudaMemcpyDeviceToDevice, stream)); return TSDRGPU_OK; }
 	void *scratch;
 	if ((rc = tsdrgpu_scratch(ctx, 0, sizeof(float2) * n_pow2, &scratch))) return rc;
@@ -907,8 +906,7 @@ int tsdrgpu_fft_oop_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const floa
 // CALLER owns (batch * n_pow2 complex; NULL: the context's scratch slot 0) -- for callers that run transforms on two streams at once
 int tsdrgpu_fft_batch_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, long long in_bs, float2 *out, long long out_bs,
                                float2 *scratch, unsigned long long n_pow2, unsigned batch, int inverse) {
-	int rc = ensure_table(ctx, stream);
-	if (rc) return rc;
+	int rc;
 	ARG_TRY(ctx, n_pow2 >= 2 && batch >= 1);
 	if (!scratch) {
 		void *sc;
@@ -960,22 +958,13 @@ int tsdrgpu_fft(tsdrgpu_ctx_t *ctx, void *stream, float *d_iq, uint32_t size, in
 // d_answer + b*answer_stride (floats, 2*size each).  skip_tail leaves answer[2N .. 2*size) untouched (the
 // frame-rate detector never reads lags >= N).
 // last[k] = exp(-i pi k / half (1 + eps)), k < half: the reference's final radix-2 stage of an (2 half)-point transform
-struct LastTab { int device; unsigned half; double eps; float2 *d; };
-static std::vector<LastTab> g_last_tabs;
 static int last_stage_table(tsdrgpu_ctx_t *ctx, unsigned half, double eps, const float2 **out) {
-	std::lock_guard<std::mutex> lock(g_tw_mu);
-	for (auto &t : g_last_tabs) if (t.device == ctx->device && t.half == half && t.eps == eps) { *out = t.d; return TSDRGPU_OK; }
-	std::vector<float2> h(half);
-	for (unsigned k = 0; k < half; k++) {
-		const double ang = -3.14159265358979323846 * ((double) k / (double) half) * (1.0 + eps);
-		h[k] = make_float2((float) cos(ang), (float) sin(ang));
-	}
-	LastTab t; t.device = ctx->device; t.half = half; t.eps = eps;
-	CU_TRY(ctx, cudaMalloc(&t.d, sizeof(float2) * half));
-	CU_TRY(ctx, cudaMemcpy(t.d, h.data(), sizeof(float2) * half, cudaMemcpyHostToDevice));
-	g_last_tabs.push_back(t);
-	*out = t.d;
-	return TSDRGPU_OK;
+	return fft_table(ctx, {TAB_LAST, half, 0, 0, eps}, half, [&](float2 *h) {
+		for (unsigned k = 0; k < half; k++) {
+			const double ang = -3.14159265358979323846 * ((double) k / (double) half) * (1.0 + eps);
+			h[k] = make_float2((float) cos(ang), (float) sin(ang));
+		}
+	}, out);
 }
 
 // Default path (TSDRGPU_AUTOCORR_FULL=1 opts out): both transforms of the autocorrelation at half size.  The capture and |X|/N
@@ -1009,9 +998,8 @@ static int autocorrelation_batch_half(tsdrgpu_ctx_t *ctx, cudaStream_t stream, f
 	const unsigned log2N = ilog2(N), half = (unsigned) (N >> 1);
 	double eps_all[40];
 	tsdrgpu_fft_reference_eps((int) log2N, 0, eps_all);
-	static const bool exact_dft = getenv("TSDRGPU_FFT_TRUE_DFT") != NULL;
 	const float2 *last;
-	int rc = last_stage_table(ctx, half, exact_dft ? 0.0 : eps_all[log2N - 1], &last);
+	int rc = last_stage_table(ctx, half, tsdrgpu_fft_true_dft() ? 0.0 : eps_all[log2N - 1], &last);
 	if (rc) return rc;
 	const unsigned G = autocorr_group(N, batch);
 	void *w0_ = wb.w0, *w1_ = wb.w1;
@@ -1049,8 +1037,7 @@ static int autocorrelation_batch_half(tsdrgpu_ctx_t *ctx, cudaStream_t stream, f
 static int autocorrelation_batch(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float *d_answer, long long answer_stride,
                                  const float *d_real, long long real_stride, uint32_t size, unsigned batch, bool skip_tail,
                                  WorkBufs wb = WorkBufs{NULL, NULL}) {
-	int rc = ensure_table(ctx, stream);
-	if (rc) return rc;
+	int rc;
 	const unsigned long long N = tsdrgpu_fft_getrealsize(size);
 	float2 *ans = reinterpret_cast<float2 *>(d_answer);
 	if (N == 1 || !skip_tail) {
@@ -1233,7 +1220,6 @@ static int frd_run_impl(tsdrgpu_frd_t *f, void *stream_, uint32_t samplerate, co
 	int rc;
 	if (fold) {
 		// only the two lag windows are ever read (frameratedetector.c:106-109)
-		if ((rc = ensure_table(ctx, stream))) return rc;
 		const RunningMeans rm = {f->d_p1.ptr, f->d_p2.ptr, fmin, flen, lmin, llen, first_calls};
 		if ((rc = autocorrelation_batch_half(ctx, stream, NULL, 0, d_capture, (long long) capture_stride, N, batch, &rm, wb))) return rc;
 	} else {
@@ -1605,6 +1591,7 @@ static int spectrum_build(tsdrgpu_spectrum *s, cudaStream_t stream) {
 	const size_t N = (size_t) s->spec.n;
 	const unsigned log2N = ilog2(N);
 	const AccShape a = acc_shape(log2N);
+	{ std::lock_guard<std::mutex> lock(ctx->mu); if (const int rc = pass_attrs(ctx)) return rc; }     // the occupancy below depends on it
 	const unsigned ctas = (unsigned) acc_ctas_per_sm(a.log2L, a.threads, a.smem) * (unsigned) ctx->sm_count;
 	s->rows_max = ctas / a.bundles > 0 ? ctas / a.bundles : 1;
 	s->seg_chunk = log2N <= (unsigned) FFT_MAX_LOG2L ? 0u : (unsigned) (SP_SCRATCH_POINTS / N > 0 ? SP_SCRATCH_POINTS / N : 1);
@@ -1653,7 +1640,6 @@ int tsdrgpu_spectrum_run(tsdrgpu_spectrum_t *s, void *stream_, const float *d_iq
 	if (nrep > capacity) return tsdrgpu_fail(ctx, TSDRGPU_ECAPACITY, "spectrum run: more reports than the output holds", cudaSuccess, __FILE__, __LINE__);
 	ARG_TRY(ctx, nrep == 0 || d_reports != NULL);
 	int rc;
-	if ((rc = ensure_table(ctx, stream))) return rc;
 	if (s->stale && (rc = spectrum_build(s, stream))) return rc;
 	*h_nreports = 0;
 	if (discontinuity) s->open = 0;

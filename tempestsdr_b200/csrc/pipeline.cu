@@ -22,6 +22,7 @@
 #include <math.h>
 #include <pthread.h>
 #include <deque>
+#include <memory>
 #include <vector>
 
 struct tsdrgpu_frd;
@@ -130,6 +131,16 @@ static inline size_t fmt_bytes(int fmt) { return fmt == TSDRGPU_FMT_FLOAT ? 4 : 
 
 }  // namespace
 
+// One hop of a superbandwidth round on device `dev`.  Ranks >= 1 of the sharded mode own a context, streams and an event; rank 0
+// and the one-GPU mode's hops borrow the pipeline's.  Destroyed after the group with `dev` current: streams and event, buffers, context.
+struct SbRank {
+	int dev = 0; tsdrgpu_ctx_t *ctx = nullptr; cudaStream_t stream = nullptr, copy = nullptr; cudaEvent_t ev = nullptr;
+	struct OwnCtx { tsdrgpu_ctx_t *c = nullptr; ~OwnCtx() { tsdrgpu_destroy(c); } } own;      // null: everything is borrowed
+	DeviceBuf<float> hop, hop0;                       // the hop; an owned rank's copy of hop 0, the alignment reference
+	DeviceBuf<unsigned char> raw;                     // an owned rank's raw-format staging (the others use the pipeline's d_raw[0])
+	~SbRank() { cudaSetDevice(dev); if (own.c) { if (stream) cudaStreamDestroy(stream); if (copy) cudaStreamDestroy(copy); if (ev) cudaEventDestroy(ev); } }
+};
+
 struct tsdrgpu_pipeline {
 	tsdrgpu_ctx_t *ctx;
 	tsdrgpu_pipeline_config_t cfg;
@@ -183,11 +194,10 @@ struct tsdrgpu_pipeline {
 	struct {
 		int state; int buffid; long long to_gather, gathered, in_frame, to_pause; uint32_t rate;
 		int nhops;                                    // SUPER_HOPS_TO_MAKE (superbandwidth.c:22): 4, or the number of devices when the hops are sharded
-		float *d_hops[16]; DeviceBuf<float> d_out; cudaEvent_t ev;
-		// one hop per GPU (tsdrgpu_pipeline_set_superb_devices): rank i records hop i on device dev[i]; rank 0 is this pipeline's device
-		int ndev; int dev[16]; tsdrgpu_ctx_t *rctx[16]; tsdrgpu_superb_mgpu_t *grp[16]; cudaStream_t rstream[16], rcopy[16]; cudaEvent_t rev[16];
-		void *rraw[16]; size_t rraw_cap[16];
-		float *d_hop0[16];                            // every device's copy of hop 0, the alignment reference (filled when hop 0 is complete)
+		DeviceBuf<float> d_out; cudaEvent_t ev;
+		// hop i is recorded by rank i; ndev ranks of one hop per GPU (tsdrgpu_pipeline_set_superb_devices), or 0 in the one-GPU mode
+		int ndev; std::unique_ptr<SbRank> rank[16];
+		tsdrgpu_superb_mgpu_t *grp[16];               // the sharded mode's group, one member per rank, once the hop size is known
 	} sb;
 	// delivery
 	pthread_t thread; pthread_mutex_t mu; pthread_cond_t cv_job, cv_done;
@@ -582,7 +592,27 @@ static int drain_blocks(tsdrgpu_pipeline *p) {
 
 extern "C" {
 
-static void superb_release_devices(tsdrgpu_pipeline *p);
+// the error a superbandwidth rank's own context holds (NULL: the thread's, where tsdrgpu_create leaves it), in the pipeline's
+static int rank_error(tsdrgpu_pipeline *p, tsdrgpu_ctx_t *from, int rc) { if (from != p->ctx) snprintf(p->ctx->err, sizeof p->ctx->err, "%s", tsdrgpu_last_error(from)); return rc; }
+// the sharded mode's ranks >= 1: a context of its own on devices[i], and streams and an event there (rank 0 is made with the hops)
+static int superb_ranks(tsdrgpu_pipeline *p, const int *devices, int n) {
+	for (int i = 1; i < n; i++) {
+		SbRank &r = *(p->sb.rank[i] = std::make_unique<SbRank>());
+		if (const int rc = tsdrgpu_create(&r.own.c, devices[i])) return rank_error(p, NULL, rc);
+		r.dev = devices[i]; r.ctx = r.own.c; CU_TRY(p->ctx, cudaSetDevice(r.dev));
+		CU_TRY(p->ctx, cudaStreamCreateWithFlags(&r.stream, cudaStreamNonBlocking)); CU_TRY(p->ctx, cudaStreamCreateWithFlags(&r.copy, cudaStreamNonBlocking));
+		CU_TRY(p->ctx, cudaEventCreateWithFlags(&r.ev, cudaEventDisableTiming));
+	}
+	CU_TRY(p->ctx, cudaSetDevice(p->ctx->device));
+	return TSDRGPU_OK;
+}
+// back to the one-GPU mode, stopped: the group first (its windows are cross-linked), then the ranks; ends on the pipeline's device
+static void superb_release(tsdrgpu_pipeline *p) {
+	for (auto &g : p->sb.grp) { tsdrgpu_superb_mgpu_destroy(g); g = NULL; }
+	for (auto &r : p->sb.rank) r.reset();
+	p->sb.ndev = 0; p->sb.rate = 0; p->sb.state = SB_STOPPED;
+	cudaSetDevice(p->ctx->device);
+}
 
 // the pipeline's own streams and events, for create and release alike
 static std::vector<cudaStream_t *> own_streams(tsdrgpu_pipeline *p) { return {&p->s_main, &p->s_copy, &p->s_out, &p->s_ingest}; }
@@ -613,7 +643,7 @@ static void release(tsdrgpu_pipeline *p) {
 	tsdrgpu_resampler_destroy(p->rs); tsdrgpu_framestage_destroy(p->fs); tsdrgpu_frd_destroy(p->frd); tsdrgpu_chanfilt_destroy(p->cf);
 	tsdrgpu_spectrum_destroy(p->sp);
 	for (auto &b : p->hostbufs) if (b.state == 1) { cudaHostUnregister(const_cast<void *>(b.base)); cudaGetLastError(); }
-	superb_release_devices(p);
+	superb_release(p);
 	for (cudaStream_t *s : own_streams(p)) if (*s) cudaStreamDestroy(*s);
 	if (p->s_spec) cudaStreamDestroy(p->s_spec);
 	for (cudaEvent_t *e : own_events(p)) if (*e) cudaEventDestroy(*e);
@@ -679,23 +709,12 @@ int tsdrgpu_pipeline_set_superb_devices(tsdrgpu_pipeline_t *p, const int *device
 	tsdrgpu_ctx_t *ctx = p->ctx;
 	BIND(ctx);
 	CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
-	superb_release_devices(p);
-	p->sb.state = SB_STOPPED;
+	superb_release(p);
 	if (n <= 1) return TSDRGPU_OK;
 	ARG_TRY(ctx, devices != NULL && (n == 2 || n == 4 || n == 8) && devices[0] == ctx->device);
-	p->sb.rctx[0] = ctx; p->sb.dev[0] = ctx->device; p->sb.rstream[0] = p->s_main; p->sb.rcopy[0] = p->s_copy;
-	for (int i = 1; i < n; i++) {
-		int rc = tsdrgpu_create(&p->sb.rctx[i], devices[i]);
-		if (rc) { snprintf(ctx->err, sizeof ctx->err, "%s", tsdrgpu_last_error(NULL)); p->sb.ndev = i; superb_release_devices(p); return rc; }
-		p->sb.dev[i] = devices[i];
-		cudaSetDevice(devices[i]);
-		cudaStreamCreateWithFlags(&p->sb.rstream[i], cudaStreamNonBlocking);
-		cudaStreamCreateWithFlags(&p->sb.rcopy[i], cudaStreamNonBlocking);
-		cudaEventCreateWithFlags(&p->sb.rev[i], cudaEventDisableTiming);
-	}
-	p->sb.ndev = n;
-	CU_TRY(ctx, cudaSetDevice(ctx->device));
-	return TSDRGPU_OK;
+	const int rc = superb_ranks(p, devices, n);
+	if (rc) superb_release(p); else p->sb.ndev = n;     // a failure leaves the one-GPU mode, its error text in ctx
+	return rc;
 }
 int tsdrgpu_pipeline_set_host_registration(tsdrgpu_pipeline_t *p, int on) { return update(p, true, [&](Settings &s) { s.host_register = on != 0; }); }
 int tsdrgpu_pipeline_set_retune(tsdrgpu_pipeline_t *p, tsdrgpu_retune_cb cb) { return update(p, true, [&](Settings &s) { s.retune_cb = cb; }); }
@@ -779,58 +798,37 @@ static int raw_reserve(tsdrgpu_pipeline *p, int ss, size_t bytes) {
 	return TSDRGPU_OK;
 }
 
-// the devices of the sharded mode own contexts, streams and (once the hop size is known) the superbandwidth group
-static void superb_release_devices(tsdrgpu_pipeline *p) {
-	for (int i = 0; i < p->sb.ndev; i++) {
-		if (p->sb.grp[i]) { tsdrgpu_superb_mgpu_destroy(p->sb.grp[i]); p->sb.grp[i] = NULL; }
+// H ranks' hop buffers (the borrowing ranks are made here) and, sharded, their group; the hop size is recorded once all of it exists
+static int superb_build(tsdrgpu_pipeline *p, const Settings &s, int H, bool sharded) {
+	tsdrgpu_ctx_t *ctx = p->ctx;
+	const long long in_frame = (long long) (s.samplerate_real / s.refreshrate), pairs = 10 * in_frame;     // SUPER_SAMPLES_TO_RECORD
+	CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
+	for (int i = 0; i < H; i++) {
+		if (!p->sb.rank[i]) p->sb.rank[i].reset(new SbRank{p->ctx->device, p->ctx, p->s_main, p->s_copy, p->sb.ev});
+		SbRank &r = *p->sb.rank[i];
+		CU_TRY(ctx, cudaSetDevice(r.dev)); CU_TRY(ctx, r.hop.assign(2 * (size_t) pairs));
+		if (r.own.c) CU_TRY(ctx, r.hop0.assign(2 * (size_t) pairs));
 	}
-	for (int i = 0; i < 16; i++) {
-		if (p->sb.d_hops[i]) { cudaSetDevice(i < p->sb.ndev ? p->sb.dev[i] : p->ctx->device); cudaFree(p->sb.d_hops[i]); p->sb.d_hops[i] = NULL; }
-		if (p->sb.rraw[i]) { cudaSetDevice(p->sb.dev[i]); cudaFree(p->sb.rraw[i]); p->sb.rraw[i] = NULL; p->sb.rraw_cap[i] = 0; }
-		if (p->sb.d_hop0[i]) { cudaSetDevice(p->sb.dev[i]); cudaFree(p->sb.d_hop0[i]); p->sb.d_hop0[i] = NULL; }
+	if (sharded) {
+		for (int i = 0; i < H; i++) { tsdrgpu_superb_mgpu_destroy(p->sb.grp[i]); p->sb.grp[i] = NULL; }
+		for (int i = 0; i < H; i++)
+			if (const int rc = tsdrgpu_superb_mgpu_create(p->sb.rank[i]->ctx, H, i, 0, (uint32_t) pairs, &p->sb.grp[i])) return rank_error(p, p->sb.rank[i]->ctx, rc);
+		if (const int rc = tsdrgpu_superb_mgpu_connect_local(p->sb.grp, H)) return rc;
 	}
-	for (int i = 1; i < p->sb.ndev; i++) {
-		cudaSetDevice(p->sb.dev[i]);
-		if (p->sb.rstream[i]) cudaStreamDestroy(p->sb.rstream[i]);
-		if (p->sb.rcopy[i]) cudaStreamDestroy(p->sb.rcopy[i]);
-		if (p->sb.rev[i]) cudaEventDestroy(p->sb.rev[i]);
-		if (p->sb.rctx[i]) tsdrgpu_destroy(p->sb.rctx[i]);
-		p->sb.rstream[i] = NULL; p->sb.rcopy[i] = NULL; p->sb.rev[i] = NULL; p->sb.rctx[i] = NULL;
-	}
-	p->sb.ndev = 0; p->sb.rate = 0;
-	cudaSetDevice(p->ctx->device);
+	CU_TRY(ctx, cudaSetDevice(ctx->device));
+	p->sb.rate = s.samplerate_real; p->sb.nhops = H; p->sb.in_frame = in_frame; p->sb.to_gather = pairs;
+	p->sb.to_pause = (long long) (0.5 * s.samplerate_real);   // SUPER_SECS_TO_PAUSE
+	return TSDRGPU_OK;
 }
 
 static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq, int fmt, uint64_t items_count, int64_t dropped) {
 	tsdrgpu_ctx_t *ctx = p->ctx;
 	int rc;
-	const int H = p->sb.ndev > 1 ? p->sb.ndev : 4;                    // SUPER_HOPS_TO_MAKE
-	const bool sharded = p->sb.ndev > 1;
+	const bool sharded = p->sb.ndev > 1; const int H = sharded ? p->sb.ndev : 4;       // SUPER_HOPS_TO_MAKE
 	if (p->sb.state == SB_STOPPED) p->sb.state = SB_STARTING;
 	if (p->sb.state == SB_STARTING) {
 		p->sb.buffid = 0; p->sb.gathered = 0;
-		if (s.samplerate_real != p->sb.rate || p->sb.nhops != H) {
-			p->sb.rate = s.samplerate_real; p->sb.nhops = H;
-			p->sb.in_frame = (long long) (s.samplerate_real / s.refreshrate);
-			p->sb.to_gather = 10 * p->sb.in_frame;                    // SUPER_SAMPLES_TO_RECORD
-			p->sb.to_pause = (long long) (0.5 * s.samplerate_real);   // SUPER_SECS_TO_PAUSE
-			CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
-			for (int i = 0; i < 16; i++) if (p->sb.d_hops[i]) { CU_TRY(ctx, cudaSetDevice(sharded && i < H ? p->sb.dev[i] : ctx->device)); CU_TRY(ctx, cudaFree(p->sb.d_hops[i])); p->sb.d_hops[i] = NULL; }
-			for (int i = 0; i < H; i++) {
-				CU_TRY(ctx, cudaSetDevice(sharded ? p->sb.dev[i] : ctx->device));
-				CU_TRY(ctx, cudaMalloc(&p->sb.d_hops[i], sizeof(float) * 2 * (size_t) p->sb.to_gather));
-				if (p->sb.d_hop0[i]) { CU_TRY(ctx, cudaFree(p->sb.d_hop0[i])); p->sb.d_hop0[i] = NULL; }
-				if (sharded && i > 0) CU_TRY(ctx, cudaMalloc(&p->sb.d_hop0[i], sizeof(float) * 2 * (size_t) p->sb.to_gather));
-			}
-			CU_TRY(ctx, cudaSetDevice(ctx->device));
-			if (sharded) {                                            // (re)build the group for this hop size
-				for (int i = 0; i < H; i++) if (p->sb.grp[i]) { tsdrgpu_superb_mgpu_destroy(p->sb.grp[i]); p->sb.grp[i] = NULL; }
-				for (int i = 0; i < H; i++)
-					if ((rc = tsdrgpu_superb_mgpu_create(p->sb.rctx[i], H, i, 0, (uint32_t) p->sb.to_gather, &p->sb.grp[i]))) { snprintf(ctx->err, sizeof ctx->err, "%s", tsdrgpu_last_error(p->sb.rctx[i])); return rc; }
-				if ((rc = tsdrgpu_superb_mgpu_connect_local(p->sb.grp, H))) { snprintf(ctx->err, sizeof ctx->err, "%s", tsdrgpu_last_error(p->sb.rctx[0])); return rc; }
-				CU_TRY(ctx, cudaSetDevice(ctx->device));
-			}
-		}
+		if ((s.samplerate_real != p->sb.rate || p->sb.nhops != H) && (rc = superb_build(p, s, H, sharded))) { cudaSetDevice(ctx->device); return rc; }
 		p->sb.state = SB_GATHERING;
 	}
 	if (p->sb.state == SB_PAUSE) {
@@ -842,24 +840,22 @@ static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq,
 	const long long now = (long long) (items_count / 2);
 	const long long take = (p->sb.gathered + now < p->sb.to_gather) ? now : (p->sb.to_gather - p->sb.gathered);
 	if (take > 0) {
-		const int b = p->sb.buffid;
-		float *hop = p->sb.d_hops[b] + 2 * p->sb.gathered;
+		SbRank &r = *p->sb.rank[p->sb.buffid];
+		float *hop = r.hop.ptr + 2 * p->sb.gathered;
 		const size_t bytes = fmt_bytes(fmt) * 2 * (size_t) take;
-		// hop b lives on the device that will transform it: the block goes there straight from the host
-		cudaStream_t cs = (sharded && b > 0) ? p->sb.rcopy[b] : p->s_copy;
-		if (sharded && b > 0) CU_TRY(ctx, cudaSetDevice(p->sb.dev[b]));
-		cudaError_t e = cudaStreamWaitEvent(cs, (sharded && b > 0) ? p->sb.rev[b] : p->sb.ev, 0);     // the last stitch has finished reading the hop buffer
+		// the hop lives on the device that will transform it: the block goes there straight from the host
+		CU_TRY(ctx, cudaSetDevice(r.dev));
+		cudaError_t e = cudaStreamWaitEvent(r.copy, r.ev, 0);     // the last stitch has finished reading the hop buffer
 		if (e == cudaSuccess) {
-			if (fmt == TSDRGPU_FMT_FLOAT) e = cudaMemcpyAsync(hop, h_iq, bytes, cudaMemcpyHostToDevice, cs);
+			if (fmt == TSDRGPU_FMT_FLOAT) e = cudaMemcpyAsync(hop, h_iq, bytes, cudaMemcpyHostToDevice, r.copy);
 			else {
-				if (sharded && b > 0 && p->sb.rraw_cap[b] < bytes) { cudaStreamSynchronize(cs); if (p->sb.rraw[b]) cudaFree(p->sb.rraw[b]); p->sb.rraw[b] = NULL; e = cudaMalloc(&p->sb.rraw[b], bytes + bytes / 2); p->sb.rraw_cap[b] = (e == cudaSuccess) ? bytes + bytes / 2 : 0; }
-				if (!(sharded && b > 0) && p->d_raw[0].cap < bytes) { cudaStreamSynchronize(cs); e = p->d_raw[0].assign(bytes + bytes / 2); }
-				void *raw = (sharded && b > 0) ? p->sb.rraw[b] : p->d_raw[0].ptr;
-				if (e == cudaSuccess) e = cudaMemcpyAsync(raw, h_iq, bytes, cudaMemcpyHostToDevice, cs);
-				if (e == cudaSuccess) { pl_convert<<<1024, 256, 0, cs>>>(raw, hop, 2 * (size_t) take, fmt); ctx->launches++; e = cudaGetLastError(); }
+				DeviceBuf<unsigned char> &raw = r.own.c ? r.raw : p->d_raw[0];
+				if (raw.cap < bytes) { cudaStreamSynchronize(r.copy); e = raw.assign(bytes + bytes / 2); }
+				if (e == cudaSuccess) e = cudaMemcpyAsync(raw.ptr, h_iq, bytes, cudaMemcpyHostToDevice, r.copy);
+				if (e == cudaSuccess) { pl_convert<<<1024, 256, 0, r.copy>>>(raw.ptr, hop, 2 * (size_t) take, fmt); ctx->launches++; e = cudaGetLastError(); }
 			}
 		}
-		const cudaError_t e2 = cudaStreamSynchronize(cs);            // the plugin's buffer has been read, whatever happened
+		const cudaError_t e2 = cudaStreamSynchronize(r.copy);            // the plugin's buffer has been read, whatever happened
 		cudaSetDevice(ctx->device);
 		if (e != cudaSuccess || e2 != cudaSuccess) return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "H2D of a superbandwidth hop block", e != cudaSuccess ? e : e2, __FILE__, __LINE__);
 		p->stats.h2d_bytes += bytes;
@@ -872,10 +868,11 @@ static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq,
 		// hop 0 is complete: every other device gets its copy now (NVLink peer copy, seconds before the stitch needs it), so that
 		// each rank derives its alignment lag from local data (superb_mgpu.cu phase 2)
 		for (int i = 1; i < H; i++) {
-			cudaSetDevice(p->sb.dev[i]);
-			cudaError_t e = cudaStreamWaitEvent(p->sb.rcopy[i], p->sb.rev[i], 0);
-			if (e == cudaSuccess) e = cudaMemcpyPeerAsync(p->sb.d_hop0[i], p->sb.dev[i], p->sb.d_hops[0], p->sb.dev[0], sizeof(float) * 2 * (size_t) count_pairs, p->sb.rcopy[i]);
-			if (e == cudaSuccess) e = cudaStreamSynchronize(p->sb.rcopy[i]);
+			SbRank &r = *p->sb.rank[i], &r0 = *p->sb.rank[0];
+			cudaSetDevice(r.dev);
+			cudaError_t e = cudaStreamWaitEvent(r.copy, r.ev, 0);
+			if (e == cudaSuccess) e = cudaMemcpyPeerAsync(r.hop0.ptr, r.dev, r0.hop.ptr, r0.dev, sizeof(float) * 2 * (size_t) count_pairs, r.copy);
+			if (e == cudaSuccess) e = cudaStreamSynchronize(r.copy);
 			if (e != cudaSuccess) { cudaSetDevice(ctx->device); return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "peer copy of the alignment reference (hop 0)", e, __FILE__, __LINE__); }
 		}
 		cudaSetDevice(ctx->device);
@@ -892,7 +889,9 @@ static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq,
 	if (!sharded) {
 		if (p->sb.d_out.cap < 2 * (size_t) H * N) { CU_TRY(ctx, cudaStreamSynchronize(p->s_main)); CU_TRY(ctx, p->sb.d_out.assign(2 * (size_t) H * N)); }
 		int offs[16], total = 0;
-		if ((rc = tsdrgpu_superb_stitch(ctx, p->s_main, p->sb.d_hops, H, (int) count_pairs, (int) p->sb.in_frame, p->sb.d_out.ptr, offs, &total))) return rc;
+		float *hops[16];
+		for (int i = 0; i < H; i++) hops[i] = p->sb.rank[i]->hop.ptr;
+		if ((rc = tsdrgpu_superb_stitch(ctx, p->s_main, hops, H, (int) count_pairs, (int) p->sb.in_frame, p->sb.d_out.ptr, offs, &total))) return rc;
 		CU_TRY(ctx, cudaEventRecord(p->sb.ev, p->s_main));
 		float *where;
 		if ((rc = decim_set_elem(p, 2))) return rc;
@@ -906,11 +905,11 @@ static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq,
 		float *where;
 		if ((rc = decim_set_elem(p, 1))) return rc;
 		if ((rc = decim_reserve(p, (size_t) H * N, &where))) return rc;
-		for (int r = 0; r < H; r++) {
-			uint32_t n = 0;
-			rc = tsdrgpu_superb_mgpu_stitch(p->sb.grp[r], r == 0 ? p->s_main : p->sb.rstream[r], p->sb.d_hops[r], r == 0 ? p->sb.d_hops[0] : p->sb.d_hop0[r], (int) count_pairs, (int) p->sb.in_frame, r == 0 ? where : NULL, &n);
-			if (rc) { snprintf(ctx->err, sizeof ctx->err, "%s", tsdrgpu_last_error(p->sb.rctx[r])); cudaSetDevice(ctx->device); return rc; }
-			if (r > 0) { cudaSetDevice(p->sb.dev[r]); cudaEventRecord(p->sb.rev[r], p->sb.rstream[r]); }
+		for (int i = 0; i < H; i++) {
+			SbRank &r = *p->sb.rank[i];
+			rc = tsdrgpu_superb_mgpu_stitch(p->sb.grp[i], r.stream, r.hop.ptr, i == 0 ? r.hop.ptr : r.hop0.ptr, (int) count_pairs, (int) p->sb.in_frame, i == 0 ? where : NULL, NULL);
+			if (rc) { cudaSetDevice(ctx->device); return rank_error(p, r.ctx, rc); }
+			if (i > 0) { cudaSetDevice(r.dev); cudaEventRecord(r.ev, r.stream); }
 		}
 		CU_TRY(ctx, cudaSetDevice(ctx->device));
 		CU_TRY(ctx, cudaEventRecord(p->sb.ev, p->s_main));

@@ -345,7 +345,7 @@ int tsdrgpu_superb_mgpu_connect_local(tsdrgpu_superb_mgpu_t *const *all, int nra
 // module loading the FIRST launch of a kernel may synchronise the whole context, and a context that holds a kernel spinning
 // on a flag which only work not yet enqueued can raise would never drain (all ranks of one process on one device, or the
 // host thread that drives every device in turn).  So the transforms of this size run once on dummy data -- which also builds
-// their twiddle tables (cudaMalloc + cudaMemcpy) and sizes the scratch -- and the small kernels are touched by name.
+// the context's own twiddle tables for them (cudaMalloc + cudaMemcpy) and sizes the scratch -- and the small kernels are touched by name.
 }  // extern "C"
 template <typename K> static void preload(K kernel) { cudaFuncAttributes a; cudaFuncGetAttributes(&a, kernel); cudaGetLastError(); }
 extern "C" {
@@ -447,8 +447,7 @@ int tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stream_, const fl
 		double eps_all[40];
 		unsigned log2N = 0; while ((1u << log2N) < N) log2N++;
 		tsdrgpu_fft_reference_eps((int) (log2N + (unsigned) g->log2H), 1, eps_all);
-		static const bool exact_dft = getenv("TSDRGPU_FFT_TRUE_DFT") != NULL;
-		for (int sidx = 0; sidx < 4; sidx++) A.eps[sidx] = (!exact_dft && sidx < g->log2H) ? eps_all[log2N + sidx] : 0.0;
+		for (int sidx = 0; sidx < 4; sidx++) A.eps[sidx] = (!tsdrgpu_fft_true_dft() && sidx < g->log2H) ? eps_all[log2N + sidx] : 0.0;
 		const unsigned grid = grid_for(N / H, ctx->sm_count, 16);
 		switch (H) {
 		case 2: KL(ctx, "sbm_final", stream, sbm_final<2><<<grid, 256, 0, stream>>>(A)); break;
