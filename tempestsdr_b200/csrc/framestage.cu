@@ -30,8 +30,8 @@ namespace cg = cooperative_groups;
 
 namespace {
 
-constexpr int FS_MAX_STRIP = 8192;      // longest width/height the in-CTA sync search supports
-constexpr int FS_MM_CHUNKS = 64;        // partial reductions per frame
+constexpr int FS_SMEM_STRIPS = 2 * 8192 + 2;   // doubles of strip buffers (w + h + 2) the sync search keeps in shared memory at most
+constexpr int FS_MM_CHUNKS = 64;       // partial reductions per frame
 constexpr int FS_SYNC_THREADS = 512;       // half an SM's registers: it must find room beside the main stream's CTAs
 
 struct SyncState {                      // device-resident syncdetector_t + dsp_autogain_t
@@ -850,11 +850,12 @@ __device__ __forceinline__ void exp_range_add(ExpRange &r, float v) {
 }
 
 // exclusive prefix sums of data[0..n) into S[0..n] IN PLACE over the same storage shifted by one:
-// on entry buf[1..n] = data, on exit buf[i] = sum_{j<i} data[j] (buf[0] = 0).  All threads of the CTA take part.
+// on entry buf[1..n] = data, on exit buf[i] = sum_{j<i} data[j] (buf[0] = 0).  All threads of the CTA take part; buf is in
+// shared or global memory.
 __device__ void exact_prefix(double *buf, int n, double *warp_tot /* >= 32 */) {
 	const int T = blockDim.x, chunk = (n + T - 1) / T;
 	const int i0 = min((int) threadIdx.x * chunk, n), i1 = min(i0 + chunk, n);
-	double local = 0.0;                                  // every thread owns one contiguous chunk (n <= 16 * blockDim.x)
+	double local = 0.0;                                  // every thread owns one contiguous chunk of ceil(n / blockDim.x) entries
 	for (int i = i0; i < i1; i++) local += buf[1 + i];
 	// exclusive scan of `local` across the CTA
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -887,8 +888,11 @@ __device__ __forceinline__ double window_from_prefix(const double *S, int n, int
 //                  blur both strips into double, exactness certificate, exact prefix scans, strip totals -- written as
 //                  one record per frame: [x buffer: w+1][y buffer: h+1][ok_x, ok_y, total_x, total_y].  A buffer holds the
 //                  prefix sums S[0..n] when its certificate holds, otherwise the blurred strip in [1..n].
+//                  Strips too long for shared memory (w + h + 2 > FS_SMEM_STRIPS) are built in the record itself.
 //   fs_sync        (one CTA walks the frames in order: the strip size and dx carry from frame to frame): records are
-//                  prefetched into shared memory one frame ahead (cp.async), every thread scores a slice of the windows
+//                  prefetched into shared memory one frame ahead (cp.async) while two fit beside the main stream's CTAs,
+//                  the next one at the bottom of the loop while one fits, and read from global memory (L2) when none
+//                  does (nbuf = 2 / 1 / 0; the same arithmetic either way), every thread scores a slice of the windows
 //                  of every candidate strip size (serial chains first when a certificate failed), first-max reduce,
 //                  thread 0 picks the strip size and updates dx/vx and the PLL average.
 // Speculation tables.  Which strip sizes frame f tries depends on frame f-1's winner -- but the winner almost always stays where
@@ -902,9 +906,13 @@ constexpr int FS_SPEC_J = 3, FS_SPEC_MAX = 24;            // sizes cur0 + 4j, |j
 constexpr int FS_SPEC_AX = 1 + 3 * FS_SPEC_MAX;           // per axis: count, sizes[], scores[], first indices[]
 constexpr int FS_PREP_HDR = 4 + 2 * FS_SPEC_AX;
 __host__ __device__ __forceinline__ size_t fs_prep_stride(int w, int h) { return (size_t) w + h + 2 + FS_PREP_HDR; }
+// whether fs_sync_prep builds a frame's strip buffers in shared memory (then copies them to the record) or directly in the
+// global record (strips longer than shared memory holds: w + h up to the reference's 4000 x 4000 pixels)
+__host__ __device__ __forceinline__ bool fs_prep_in_smem(int w, int h) { return (size_t) w + h + 2 <= (size_t) FS_SMEM_STRIPS; }
 
 // the strip sizes a frame's search tries, in the reference's order (syncdetector.c:60-69, 73-77, 88-93); vals[t] = -1: skipped.
-// `cur` is clamped in place like the reference clamps sweetspot_data_t.curr_stripsize.
+// `cur` is clamped in place like the reference clamps sweetspot_data_t.curr_stripsize.  vals[0] is always tried, also when the
+// clamp leaves 0 (a strip of 1 pixel: half = 0): the reference then scores a zero-length strip, NaN at every start, and keeps index 0.
 __device__ __forceinline__ void sweet_candidates(int &cur, int size, int minsize, int vals[5]) {
 	if (minsize < 1) minsize = 1;
 	const int half = size >> 1;
@@ -914,19 +922,22 @@ __device__ __forceinline__ void sweet_candidates(int &cur, int size, int minsize
 	for (int t = 1; t < 5; t++) vals[t] = (tries[t] >= minsize && tries[t] < half && tries[t] != cur) ? tries[t] : -1;
 }
 
+// GREC: the strip buffers are built in the global record (!fs_prep_in_smem), not in shared memory
+template <bool GREC>
 __global__ void __launch_bounds__(FS_SYNC_THREADS) fs_sync_prep(const float *__restrict__ wstrips, const float *__restrict__ hstrips,
                                                                 int w, int h, float c0, float c1, float c2, float c3, float c4,
                                                                 int force_serial, double *__restrict__ prep,
                                                                 const SyncState *__restrict__ state, int minsize_x, int minsize_y, int spec_on) {
 	extern __shared__ double smem_d[];
-	double *buf_x = smem_d, *buf_y = buf_x + (w + 1);
+	const int f = blockIdx.x;
+	double *rec = prep + (size_t) f * fs_prep_stride(w, h);
+	double *buf_x = GREC ? rec : smem_d, *buf_y = buf_x + (w + 1);
 	__shared__ float tiny[16];
 	__shared__ double warp_tot[32];
 	__shared__ int range_lo[2], range_hi[2], range_bad[2], exact_ok[2];
 	__shared__ float totalf[2];
 	const float taps[5] = {c0, c1, c2, c3, c4};
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	const int f = blockIdx.x;
 	if (threadIdx.x < 2) { range_lo[threadIdx.x] = 255; range_hi[threadIdx.x] = 0; range_bad[threadIdx.x] = 0; }
 	if (threadIdx.x == 0) { buf_x[0] = 0.0; buf_y[0] = 0.0; }
 	blur_to_double(wstrips + (size_t) f * w, buf_x + 1, w, taps, tiny);
@@ -947,7 +958,7 @@ __global__ void __launch_bounds__(FS_SYNC_THREADS) fs_sync_prep(const float *__r
 		const int ax = threadIdx.x, n = ax ? h : w;
 		int lg = 0; while ((1 << lg) < n) lg++;
 		const int span = (range_hi[ax] >= range_lo[ax]) ? (range_hi[ax] - range_lo[ax]) : 0;
-		exact_ok[ax] = !force_serial && !range_bad[ax] && n <= 16 * (int) blockDim.x && (span < 29 - lg);
+		exact_ok[ax] = !force_serial && !range_bad[ax] && (span < 29 - lg);
 	}
 	__syncthreads();
 	const bool ok_x = exact_ok[0], ok_y = exact_ok[1];
@@ -958,9 +969,8 @@ __global__ void __launch_bounds__(FS_SYNC_THREADS) fs_sync_prep(const float *__r
 	__syncthreads();
 	if (threadIdx.x < 2 && exact_ok[threadIdx.x]) totalf[threadIdx.x] = __double2float_rn(threadIdx.x ? buf_y[h] : buf_x[w]);   // findbestfit takes a float
 	__syncthreads();
-	double *rec = prep + (size_t) f * fs_prep_stride(w, h);
 	const int nbody = w + h + 2;
-	for (int i = threadIdx.x; i < nbody; i += blockDim.x) rec[i] = smem_d[i];
+	if (!GREC) for (int i = threadIdx.x; i < nbody; i += blockDim.x) rec[i] = smem_d[i];
 	if (threadIdx.x == 0) {
 		rec[nbody + 0] = ok_x ? 1.0 : 0.0; rec[nbody + 1] = ok_y ? 1.0 : 0.0;
 		rec[nbody + 2] = (double) totalf[0]; rec[nbody + 3] = (double) totalf[1];
@@ -1082,7 +1092,7 @@ __global__ void __launch_bounds__(64) fs_sync_walk(const double *__restrict__ pr
 		bool ok = cur_t.n > 0, first = true;
 		#pragma unroll
 		for (int t = 0; t < 5; t++) {
-			if (vals[t] <= 0) continue;
+			if (vals[t] < 0) continue;
 			const unsigned hit = __ballot_sync(0xffffffffu, cur_t.sz == vals[t]);
 			if (!hit) { ok = false; continue; }
 			const int src = __ffs(hit) - 1;
@@ -1113,6 +1123,8 @@ __global__ void __launch_bounds__(64) fs_sync_walk(const double *__restrict__ pr
 // candidate sizes the same way: two cluster barriers per frame.
 constexpr int FS_SEL_THREADS = 512, FS_SEL_CLUSTER = 8, FS_SEL_WARPS = FS_SEL_THREADS / 32;
 
+// GREC: the records are read in global memory (nbuf = 0), not from shared memory
+template <bool GREC>
 __global__ void __cluster_dims__(FS_SEL_CLUSTER, 1, 1) __launch_bounds__(FS_SEL_THREADS)
 fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, int minsize_y, int nframes,
         SyncState *state, double *__restrict__ chain_scratch, tsdrgpu_frame_result_t *results, const int *__restrict__ resume) {
@@ -1129,9 +1141,11 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 	__shared__ SyncState st;                             // CTA 0
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-	// clamp the carried strip size, list the sizes to try (syncdetector.c:73-77, 60-69, 88-93), tell every CTA
+	// clamp the carried strip size, list the sizes to try (syncdetector.c:73-77, 60-69, 88-93), tell every CTA.  The clamp works on
+	// a copy: after a batch's last frame the state keeps the winner itself, as the reference does (where half < minsize, a
+	// one-pixel axis, clamping twice is not clamping once: 1 -> 0 -> 1)
 	auto list_candidates = [&](int ax) {
-		int &cur = ax ? st.y_strip : st.x_strip;
+		int cur = ax ? st.y_strip : st.x_strip;
 		int vals[5];
 		sweet_candidates(cur, ax ? h : w, ax ? minsize_y : minsize_x, vals);
 		for (unsigned r = 0; r < FS_SEL_CLUSTER; r++) {
@@ -1144,16 +1158,18 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 		__syncthreads();
 		if (threadIdx.x == 0 || threadIdx.x == 32) list_candidates(threadIdx.x >> 5);
 	}
-	fs_prefetch_record(smem_d + (size_t) (nbuf == 2 ? (f_start & 1) : 0) * rec_len, prep + (size_t) f_start * rec_len, rec_len);
+	if (!GREC) fs_prefetch_record(smem_d + (size_t) (nbuf == 2 ? (f_start & 1) : 0) * rec_len, prep + (size_t) f_start * rec_len, rec_len);
 	cluster.sync();
+	const size_t chain_len = (size_t) max(w, h);         // one window sum per start position of the longer strip (fs_reserve)
 
 	const int units_x = (w + 31) >> 5, units_y = (h + 31) >> 5, units = 5 * (units_x + units_y);
 	for (int f = f_start; f < nframes; f++) {
-		double *rec = smem_d + (size_t) (nbuf == 2 ? (f & 1) : 0) * rec_len;
+		// nbuf = 0: records longer than shared memory holds are read where fs_sync_prep left them (global memory, mostly from L2)
+		const double *rec = GREC ? prep + (size_t) f * rec_len : smem_d + (size_t) (nbuf == 2 ? (f & 1) : 0) * rec_len;
 		__pipeline_wait_prior(0);
 		__syncthreads();                                 // record f is in shared memory; the other buffer is no longer read
-		if (nbuf == 2 && f + 1 < nframes) fs_prefetch_record(smem_d + (size_t) ((f + 1) & 1) * rec_len, prep + (size_t) (f + 1) * rec_len, rec_len);
-		double *buf_x = rec, *buf_y = rec + (w + 1);     // prefix sums S[0..n], or the blurred strip in [1..n]
+		if (!GREC && nbuf == 2 && f + 1 < nframes) fs_prefetch_record(smem_d + (size_t) ((f + 1) & 1) * rec_len, prep + (size_t) (f + 1) * rec_len, rec_len);
+		const double *buf_x = rec, *buf_y = rec + (w + 1);     // prefix sums S[0..n], or the blurred strip in [1..n]
 		const bool ok_x = rec[nbody + 0] != 0.0, ok_y = rec[nbody + 1] != 0.0;
 		const float tot_x = (float) rec[nbody + 2], tot_y = (float) rec[nbody + 3];
 		// serial chains for strips that failed the certificate: chain ci on CTA ci % 8, window sums to the global scratch
@@ -1162,7 +1178,7 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 				const int ci = (int) rank + FS_SEL_CLUSTER * warp;
 				if (ci < 10) {
 					const int ax = ci / 5, strip = cand[ax][ci % 5];
-					if (strip > 0 && !(ax ? ok_y : ok_x)) window_sums((ax ? buf_y : buf_x) + 1, ax ? h : w, strip, chain_scratch + (size_t) ci * FS_MAX_STRIP);
+					if (strip >= 0 && !(ax ? ok_y : ok_x)) window_sums((ax ? buf_y : buf_x) + 1, ax ? h : w, strip, chain_scratch + (size_t) ci * chain_len);
 				}
 			}
 			cluster.sync();
@@ -1175,12 +1191,12 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 			if (u < 5 * units_x) { ci = u / units_x; blk = u - ci * units_x; }
 			else { const int u2 = u - 5 * units_x; ci = u2 / units_y; blk = u2 - ci * units_y; ci += 5; }
 			const int ax = ci / 5, strip = cand[ax][ci % 5];
-			if (strip <= 0) continue;
+			if (strip < 0) continue;
 			const int size = ax ? h : w, e = (blk << 5) + lane;
 			Best b; b.score = -INFINITY; b.e = 0x7fffffff;
 			if (e < size) {
 				const bool ok = ax ? ok_y : ok_x;
-				const double c = ok ? window_from_prefix(ax ? buf_y : buf_x, size, e, strip) : chain_scratch[(size_t) ci * FS_MAX_STRIP + e];
+				const double c = ok ? window_from_prefix(ax ? buf_y : buf_x, size, e, strip) : chain_scratch[(size_t) ci * chain_len + e];
 				const double sc = fit_score((double) (ax ? tot_y : tot_x), c, (double) (size - strip), (double) strip);
 				if (sc > b.score) { b.score = sc; b.e = e; }
 			}
@@ -1203,7 +1219,7 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 				const int ci = threadIdx.x, ax = ci / 5, t = ci % 5;
 				const int strip = cand[ax][t];
 				Best r; r.score = -1.0; r.e = -1;
-				if (strip > 0) {
+				if (strip >= 0) {
 					const int size = ax ? h : w;
 					r = rank_best[0][ci];
 					for (int k = 1; k < FS_SEL_CLUSTER; k++) r = best_merge(r, rank_best[k][ci]);
@@ -1211,7 +1227,7 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 					// (with the certificate every score is a finite square, so this only matters on the serial-chain path)
 					const bool ok = ax ? ok_y : ok_x;
 					if (!ok || r.e == 0x7fffffff) {
-						const double c0s = ok ? window_from_prefix(ax ? buf_y : buf_x, size, 0, strip) : chain_scratch[(size_t) ci * FS_MAX_STRIP];
+						const double c0s = ok ? window_from_prefix(ax ? buf_y : buf_x, size, 0, strip) : chain_scratch[(size_t) ci * chain_len];
 						const double s0 = fit_score((double) (ax ? tot_y : tot_x), c0s, (double) (size - strip), (double) strip);
 						if (!(s0 == s0) || r.e == 0x7fffffff) { r.score = s0; r.e = 0; }
 					}
@@ -1225,7 +1241,7 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 				Best best = cand_best[ax][0];
 				int best_size = cand[ax][0];
 				for (int t = 1; t < 5; t++) {
-					if (cand[ax][t] <= 0) continue;
+					if (cand[ax][t] < 0) continue;
 					if (cand_best[ax][t].score > best.score) { best = cand_best[ax][t]; best_size = cand[ax][t]; }
 				}
 				sweet_update(ax, st, best, best_size, ax ? h : w, results + f);   // the auto-gain fields of the record belong to fs_results_autogain
@@ -1233,7 +1249,7 @@ fs_sync(const double *__restrict__ prep, int nbuf, int w, int h, int minsize_x, 
 			}
 		}
 		cluster.sync();
-		if (nbuf != 2 && f + 1 < nframes) fs_prefetch_record(smem_d, prep + (size_t) (f + 1) * rec_len, rec_len);
+		if (!GREC && nbuf == 1 && f + 1 < nframes) fs_prefetch_record(smem_d, prep + (size_t) (f + 1) * rec_len, rec_len);
 	}
 	if (rank == 0 && threadIdx.x == 0) {
 		// auto-gain fields of the state are owned by the auto-gain epilogue: write back the sync part only
@@ -1380,15 +1396,16 @@ __global__ void __launch_bounds__(256) fs_argb_batch(float *frames, size_t n, in
 	}
 }
 
-__global__ void fs_blur_kernel(float *data, int n, float c0, float c1, float c2, float c3, float c4) {
+// in shared memory, or (scratch != NULL: strips too long for it) from a copy in `scratch` straight back into `data`
+__global__ void fs_blur_kernel(float *data, float *scratch, int n, float c0, float c1, float c2, float c3, float c4) {
 	extern __shared__ float smem[];
-	float *src = smem, *dst = smem + n;
+	float *src = scratch ? scratch : smem, *dst = scratch ? data : smem + n;
 	const float taps[5] = {c0, c1, c2, c3, c4};
 	for (int i = threadIdx.x; i < n; i += blockDim.x) src[i] = data[i];
 	__syncthreads();
 	blur_strip(src, dst, n, taps);
 	__syncthreads();
-	for (int i = threadIdx.x; i < n; i += blockDim.x) data[i] = dst[i];
+	if (!scratch) for (int i = threadIdx.x; i < n; i += blockDim.x) data[i] = dst[i];
 }
 
 inline unsigned grid_for(size_t n, int sm_count, int per_sm = 8) {
@@ -1537,6 +1554,8 @@ static int fs_reserve(tsdrgpu_framestage *fs, int nframes, size_t n, int w, int 
 	if ((rc = fs_assign_group(ctx, strips, (size_t) nframes * (size_t) (w > h ? w : h)))) return rc;
 	DeviceBuf<double> *const prep[] = {&fs->d_prep};
 	if ((rc = fs_assign_group(ctx, prep, (size_t) nframes * fs_prep_stride(w, h)))) return rc;
+	DeviceBuf<double> *const chain[] = {&fs->d_chain};       // fs_sync's serial chains: 10 candidates x the longer strip
+	if ((rc = fs_assign_group(ctx, chain, (size_t) 10 * (size_t) (w > h ? w : h)))) return rc;
 	if (fs->batch_cap < nframes) {
 		CU_TRY(ctx, cudaDeviceSynchronize());
 		fs->batch_cap = 0;
@@ -1614,7 +1633,6 @@ static void release(tsdrgpu_framestage *fs) {
 static int create_handles(tsdrgpu_framestage *fs) {
 	tsdrgpu_ctx_t *ctx = fs->ctx;
 	CU_TRY(ctx, fs->d_state.assign(1));
-	CU_TRY(ctx, fs->d_chain.assign(10 * FS_MAX_STRIP));
 	CU_TRY(ctx, fs->d_resume.assign(64));
 	CU_TRY(ctx, cudaMemset(fs->d_resume.ptr, 0, 256));
 	CU_TRY(ctx, fs->d_cert.assign(1));
@@ -1741,7 +1759,6 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 	cudaStream_t stream = (cudaStream_t) stream_;
 	if (nframes == 0) return TSDRGPU_OK;
 	ARG_TRY(ctx, nframes > 0 && w > 0 && h > 0 && d_in != NULL && d_out != NULL && d_in != d_out);
-	ARG_TRY(ctx, w <= FS_MAX_STRIP && h <= FS_MAX_STRIP);
 	const size_t n = (size_t) w * h;
 	const bool autoshift = flags & TSDRGPU_FS_AUTOSHIFT, lpbs = flags & TSDRGPU_FS_LOWPASS_BEFORE_SYNC;
 	const bool aap = flags & TSDRGPU_FS_AUTOGAIN_AFTER_PROC, superres = flags & TSDRGPU_FS_SUPERRESOLUTION;
@@ -1782,12 +1799,15 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 	tsdrgpu_frame_result_t *d_results = fs->d_results[ph].ptr;
 	const double fresh = 1.0 - (double) motionblur;      // dsp.c:29
 	const int minsize_x = (int) (w * 0.05f), minsize_y = (int) (h * 0.01f);   // syncdetector.c:178-179
-	const size_t prep_smem = sizeof(double) * ((size_t) w + h + 2);
+	const size_t prep_smem = fs_prep_in_smem(w, h) ? sizeof(double) * ((size_t) w + h + 2) : 0;
 	const size_t rec_bytes = sizeof(double) * fs_prep_stride(w, h);
-	const int sync_nbuf = (2 * rec_bytes <= 96 * 1024) ? 2 : 1;     // prefetch one frame ahead while two records fit beside the main stream's CTAs
+	const size_t rec_smem_max = sizeof(double) * (FS_SMEM_STRIPS + FS_PREP_HDR);
+	// prefetch one frame ahead while two records fit beside the main stream's CTAs, else one record at a time while one fits in
+	// shared memory, else read them in global memory
+	const int sync_nbuf = (2 * rec_bytes <= 96 * 1024) ? 2 : (rec_bytes <= rec_smem_max ? 1 : 0);
 	const size_t sync_smem = rec_bytes * sync_nbuf;
-	CU_TRY(ctx, cudaFuncSetAttribute(fs_sync_prep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (sizeof(double) * (2 * FS_MAX_STRIP + 2))));
-	CU_TRY(ctx, cudaFuncSetAttribute(fs_sync, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (sizeof(double) * (2 * FS_MAX_STRIP + 2 + FS_PREP_HDR))));
+	CU_TRY(ctx, cudaFuncSetAttribute(fs_sync_prep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (sizeof(double) * FS_SMEM_STRIPS)));
+	CU_TRY(ctx, cudaFuncSetAttribute(fs_sync<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) rec_smem_max));
 	const int force_serial = getenv("TSDRGPU_SYNC_SERIAL") ? 1 : 0;      // test hook: always take the serial-chain path
 	const unsigned gx = grid_for(n, ctx->sm_count, 4);
 	const size_t total = (size_t) nframes * n;
@@ -1800,10 +1820,13 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 			CU_TRY(ctx, cudaStreamWaitEvent(s2, fs->ev_ready[ph], 0));
 		}
 		static const bool no_spec = getenv("TSDRGPU_SYNC_NO_SPEC") != NULL;      // test hook: always the literal cluster search
-		KL(ctx, "fs_sync_prep", s2, fs_sync_prep<<<nframes, FS_SYNC_THREADS, prep_smem, s2>>>(fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, w, h,
+		auto prep_kernel = fs_prep_in_smem(w, h) ? fs_sync_prep<false> : fs_sync_prep<true>;
+		KL(ctx, "fs_sync_prep", s2, prep_kernel<<<nframes, FS_SYNC_THREADS, prep_smem, s2>>>(fs->d_wstrips[ph].ptr, fs->d_hstrips[ph].ptr, w, h,
 			fs->taps[0], fs->taps[1], fs->taps[2], fs->taps[3], fs->taps[4], force_serial, fs->d_prep.ptr, fs->d_state.ptr, minsize_x, minsize_y, no_spec ? 0 : 1));
 		KL(ctx, "fs_sync_walk", s2, fs_sync_walk<<<1, 64, 0, s2>>>(fs->d_prep.ptr, w, h, minsize_x, minsize_y, nframes, fs->d_state.ptr, d_results, fs->d_resume.ptr));
-		KL(ctx, "fs_sync", s2, fs_sync<<<FS_SEL_CLUSTER, FS_SEL_THREADS, sync_smem, s2>>>(fs->d_prep.ptr, sync_nbuf, w, h, minsize_x, minsize_y, nframes,
+		if (sync_nbuf) KL(ctx, "fs_sync", s2, fs_sync<false><<<FS_SEL_CLUSTER, FS_SEL_THREADS, sync_smem, s2>>>(fs->d_prep.ptr, sync_nbuf, w, h, minsize_x, minsize_y, nframes,
+			fs->d_state.ptr, fs->d_chain.ptr, d_results, fs->d_resume.ptr));
+		else KL(ctx, "fs_sync", s2, fs_sync<true><<<FS_SEL_CLUSTER, FS_SEL_THREADS, 0, s2>>>(fs->d_prep.ptr, 0, w, h, minsize_x, minsize_y, nframes,
 			fs->d_state.ptr, fs->d_chain.ptr, d_results, fs->d_resume.ptr));
 		return TSDRGPU_OK;
 	};
@@ -1977,12 +2000,20 @@ int tsdrgpu_average_v_h(tsdrgpu_ctx_t *ctx, void *stream, int w, int h, const fl
 
 int tsdrgpu_gaussianblur(tsdrgpu_ctx_t *ctx, void *stream, float *d_data, int n) {
 	BIND(ctx);
-	ARG_TRY(ctx, n > 0 && n <= 2 * FS_MAX_STRIP && d_data);
+	ARG_TRY(ctx, n > 0 && d_data);
 	float t[5];
 	tsdrgpu_gauss_taps(t);
-	CU_TRY(ctx, cudaFuncSetAttribute(fs_blur_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) (sizeof(float) * 4 * FS_MAX_STRIP)));
-	fs_blur_kernel<<<1, 256, sizeof(float) * 2 * n, (cudaStream_t) stream>>>(d_data, n, t[0], t[1], t[2], t[3], t[4]);
-	LAUNCH_CHECK(ctx);
+	constexpr int smem_n = 2 * 8192;                     // strips kept in shared memory (source and result: 128 KB)
+	const int smem_max = (int) (sizeof(float) * 2 * smem_n);
+	const bool in_smem = n <= smem_n;
+	CU_TRY(ctx, cudaFuncSetAttribute(fs_blur_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+	float *scratch = NULL;                               // longer strips: a copy on the stream, allocated and freed in stream order
+	if (!in_smem) CU_TRY(ctx, cudaMallocAsync((void **) &scratch, sizeof(float) * (size_t) n, (cudaStream_t) stream));
+	fs_blur_kernel<<<1, 256, in_smem ? sizeof(float) * 2 * n : 0, (cudaStream_t) stream>>>(d_data, scratch, n, t[0], t[1], t[2], t[3], t[4]);
+	const cudaError_t launched = cudaGetLastError();
+	if (scratch) CU_TRY(ctx, cudaFreeAsync(scratch, (cudaStream_t) stream));
+	if (launched != cudaSuccess) return tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "kernel launch", launched, __FILE__, __LINE__);
+	ctx->launches++;
 	return TSDRGPU_OK;
 }
 

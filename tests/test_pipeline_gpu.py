@@ -11,15 +11,36 @@ from tempestsdr_b200 import synth
 pytestmark = pytest.mark.gpu
 
 
-def run_oracle_stream(O, iq_blocks, fs, h, fv, plots=True):
-    """Single-threaded replay of process() -> decimatingthread -> postprocessingthread with the reference stages."""
+class StaleZeroResampler:
+    """The oracle's resampler with the slot the reference leaves stale set to 0.0f, as the CUDA path writes it (DESIGN.md §2: when
+    (size - offset) * r lands exactly on an integer the reference's loop writes one pixel fewer than it sizes its output for, and
+    that slot keeps stale buffer content).  The pinned restatement runs beside it on the same blocks to say where that happens."""
+
+    def __init__(self, O):
+        self.rs, self.port = O.resampler(), orc.port().resampler()
+
+    def run(self, x, up, down):
+        out = self.rs.run(x, up, down)
+        self.port.run(x, up, down)
+        out[self.port.last_emitted:] = 0.0
+        return out
+
+
+def run_oracle_stream(O, iq_blocks, fs, h, fv, plots=True, resolutions=None):
+    """Single-threaded replay of process() -> decimatingthread -> postprocessingthread with the reference stages.
+    resolutions: {index of an IQ block: (height, refresh rate)} set before that block is processed (set_resolution between
+    process() calls): groups of ten decimator blocks resampled after it use the new geometry, and frames are cut with the
+    geometry of the group that completed them, pixels left from the old geometry included.  Returns (width at the end, frames)."""
     w, _, _ = O.geometry(fs, h, fv)
-    n = w * h
-    block = int(0.1 * fs / fv)
-    rs = O.resampler(); pp = O.postprocessor(fs, h, fv, 1, 0)
+    rs = StaleZeroResampler(O); pp = O.postprocessor(fs, h, fv, 1, 0)
     decim = np.zeros(0, np.float32); pix = np.zeros(0, np.float32)
     frames = []
-    for iq in iq_blocks:
+    for i, iq in enumerate(iq_blocks):
+        if resolutions and i in resolutions:
+            h, fv = resolutions[i]
+            w, _, _ = O.geometry(fs, h, fv)
+        n = w * h
+        block = int(0.1 * fs / fv)
         decim = np.concatenate([decim, O.am_demod(iq)])
         while decim.size >= 10 * block:
             for k in range(10):
