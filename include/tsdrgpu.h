@@ -465,6 +465,52 @@ TSDRGPU_API int  tsdrgpu_denoise_parse(const char *spec, int *mode, int *h_milli
 TSDRGPU_API int  tsdrgpu_nlm(tsdrgpu_ctx_t *ctx, void *stream, const float *d_in, float *d_out, int w, int h, int nframes,
                              int h_milli, int r, int p);
 
+/* ---------------------------------------------------------------------------- a8+  Richardson-Lucy deconvolution along the lines (beyond the reference)
+ * Every geometry decodes at about two pixels per IQ sample (W = (int)(2 fs / (fv h))), and the front end has already averaged the
+ * signal over the sample period, so a one-pixel stroke comes out as a bump about three pixels wide.  On one frame that is aliasing
+ * as well as blur, but an average of frames whose sampling phase drifts (the stack, or motion blur > 0) is the picture convolved
+ * with a fixed line-spread function, which deconvolution can undo.  It runs on each frame as delivered, after the stack and before
+ * NLM and CLAHE (stack -> deblur -> NLM -> CLAHE; RL assumes a linear blur, which NLM's weights are not), and never feeds back:
+ * d_screen, lastmin/lastmax, the sync state and every tsdrgpu_frame_result_t field are unchanged.
+ * Each line y of a frame is processed on its own (lines are separate in time; after the re-centring the blanking sits at the line
+ * ends, so there is no vertical blur to undo).  sigma = sigma_centi / 100 in [0.25, 4] pixels, iterations I in [1, 64]:
+ *   1. taps: R = ceil(3 sigma) = (3 sigma_centi + 99) / 100 in integers; k_j = exp(-j^2 / (2 sigma^2)) / sum, j in [-R, R], the sum
+ *      over the same j, all in double, each tap rounded once to float (tsdrgpu_deblur_taps).
+ *   2. inputs: valid(v) is !(v > 250 || v < -250) && v == v; m(x) = valid as 0 / 1, and a position outside the line counts as
+ *      invalid, so line ends and markers follow one rule.  d(x) = m ? (v > 0 ? min(v, 1) : 0) : 0 (the clamp to [0, 1], with -0
+ *      taken to +0).
+ *   3. masked correlation: B(a)(x) = sum_j k_j (m(x+j) a(x+j)), j from -R to R, left to right, each product and sum rounded to
+ *      float32.  rn(x) = 1.0f / B(1)(x), one IEEE division, once per line, where m = 1 (there B(1) >= k_0 > 0).
+ *   4. iterations: u_0 = d; each iteration, per pixel: b = B(u) rn; q = m ? d / max(b, eps) : 0; u <- m ? u (B(q) rn) : 0, with
+ *      eps = TSDRGPU_DEBLUR_EPS (2^-30), every operation rounded to float32, no contraction, IEEE division.
+ *   5. output: out = valid(v) ? min(u_I, 1.0f) : v.  Markers, NaN and +-inf pass through in place; valid outputs lie in [0, 1],
+ *      so NLM, CLAHE, tsdrgpu_pixels_argb and the ARGB pipeline output apply unchanged.
+ * A valid pixel further than 2 R I pixels from every invalid pixel and line end is unaffected by them.
+ * Guidance: sigma near 1 fits the box resampler (its ratio r = pixelrate / fs is within 0.2 % of 2, and the two r-pixel boxes of
+ * integration and hold give r / sqrt(6) = 0.82, to which the front end's own roll-off adds); the sinc resampler wants less.  The
+ * step is meant for averaged frames (the stack, or motion blur > 0): on a single noisy frame it amplifies noise and aliasing. */
+enum { TSDRGPU_DEBLUR_OFF = 0, TSDRGPU_DEBLUR_RL = 1 };
+#define TSDRGPU_DEBLUR_MIN_SIGMA 25           /* sigma_centi */
+#define TSDRGPU_DEBLUR_MAX_SIGMA 400
+#define TSDRGPU_DEBLUR_MAX_ITER  64
+#define TSDRGPU_DEBLUR_MAX_R     12           /* ceil(3 * 4) */
+#define TSDRGPU_DEBLUR_EPS       0x1p-30f
+/* host-only: the taps of step 1.  *R (may be NULL) receives R; taps (may be NULL) receives the 2R + 1 taps k_{-R} .. k_R.
+ * TSDRGPU_EINVAL for sigma_centi outside [25, 400]. */
+TSDRGPU_API int  tsdrgpu_deblur_taps(int sigma_centi, float *taps, int *R);
+/* the frame stage's deblur mode, applied from the next run on and kept across tsdrgpu_framestage_reset.  With
+ * TSDRGPU_DEBLUR_OFF (the default) the other arguments are ignored.  Out-of-range values or an unknown mode: TSDRGPU_EINVAL. */
+TSDRGPU_API int  tsdrgpu_framestage_set_deblur(tsdrgpu_framestage_t *fs, int mode, int sigma_centi, int iterations);
+/* host-only: the spelling shared by the host library's TSDR_DEBLUR and Python.  "off", "rl:<sigma>" or "rl:<sigma>:<I>";
+ * sigma = one to six digits, optionally '.' and one or two digits, value in [0.25, 4], converted to hundredths with integer
+ * arithmetic; I = one to six digits in [1, 64], default 20.  Nothing else (no sign, blank or exponent).
+ * TSDRGPU_OK with the three outputs set (zeros for "off"), else TSDRGPU_EINVAL and the outputs untouched. */
+TSDRGPU_API int  tsdrgpu_deblur_parse(const char *spec, int *mode, int *sigma_centi, int *iterations);
+/* stage level (synchronises): deblur of nframes frames of w x h (w h <= TSDRGPU_MAX_FRAME_PIXELS) back to back from d_in to
+ * d_out, both 4-byte aligned.  It cannot run in place: overlapping buffers are refused with TSDRGPU_EINVAL. */
+TSDRGPU_API int  tsdrgpu_deblur(tsdrgpu_ctx_t *ctx, void *stream, const float *d_in, float *d_out, int w, int h, int nframes,
+                                int sigma_centi, int iterations);
+
 /* ---------------------------------------------------------------------------- a8+  drift-registered frame averaging (beyond the reference)
  * Averaging many frames is how faint text is read, but the reference's temporal IIR (motionblur, dsp.c:22-33) averages in raster
  * coordinates before the sync search re-centres the frame, so any drift of the picture between frames is averaged in as smear.
@@ -769,6 +815,9 @@ TSDRGPU_API int  tsdrgpu_pipeline_set_contrast(tsdrgpu_pipeline_t *p, int mode, 
 /* denoise mode (TSDRGPU_DENOISE_OFF, the default, or TSDRGPU_DENOISE_NLM; see tsdrgpu_framestage_set_denoise), taking effect
  * at the next frame-stage batch */
 TSDRGPU_API int  tsdrgpu_pipeline_set_denoise(tsdrgpu_pipeline_t *p, int mode, int h_milli, int r, int p_radius);
+/* deblur mode (TSDRGPU_DEBLUR_OFF, the default, or TSDRGPU_DEBLUR_RL; see tsdrgpu_framestage_set_deblur), taking effect at the
+ * next frame-stage batch */
+TSDRGPU_API int  tsdrgpu_pipeline_set_deblur(tsdrgpu_pipeline_t *p, int mode, int sigma_centi, int iterations);
 /* stack mode (TSDRGPU_STACK_OFF, the default, TSDRGPU_STACK_ALIGN or TSDRGPU_STACK_ADAPT; see tsdrgpu_framestage_set_stack),
  * taking effect at the next frame-stage batch.  tsdrgpu_pipeline_sync restarts the stack at the next frame-stage batch.  While
  * the stack is on, every frame with an auto-gain report (dsp.c:231-235) also announces value id TSDRGPU_VALUE_ID_STACK_DRIFT with arg0 = the mean drift

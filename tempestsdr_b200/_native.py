@@ -115,6 +115,18 @@ def denoise_mode(spec: str):
     return tuple(o.value for o in out)
 
 
+DEBLUR_OFF, DEBLUR_RL = 0, 1                       # TSDRGPU_DEBLUR_OFF / TSDRGPU_DEBLUR_RL
+
+
+def deblur_mode(spec: str):
+    """"off", "rl:<sigma>" or "rl:<sigma>:<I>" (the host library's TSDR_DEBLUR spelling) -> (mode, sigma_centi, I), read by
+    tsdrgpu_deblur_parse."""
+    out = [C.c_int() for _ in range(3)]
+    if lib().tsdrgpu_deblur_parse(spec.encode(), *[C.byref(o) for o in out]) != 0:
+        raise ValueError(f"deblur must be 'off' or 'rl:<sigma>[:<I>]' with sigma in [0.25, 4] and I in [1, 64], not {spec!r}")
+    return tuple(o.value for o in out)
+
+
 STACK_OFF, STACK_ALIGN, STACK_ADAPT = 0, 1, 4      # TSDRGPU_STACK_OFF / TSDRGPU_STACK_ALIGN / TSDRGPU_STACK_ADAPT
 VALUE_ID_STACK_DRIFT = 101                          # TSDRGPU_VALUE_ID_STACK_DRIFT
 
@@ -207,6 +219,10 @@ _SIGS = {
     "tsdrgpu_framestage_set_denoise": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_denoise_parse": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "tsdrgpu_nlm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "tsdrgpu_deblur_parse": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "tsdrgpu_deblur_taps": (C.c_int, [C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
+    "tsdrgpu_deblur": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "tsdrgpu_framestage_set_deblur": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_stack_parse": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "tsdrgpu_stack_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "tsdrgpu_stack_destroy": (None, [C.c_void_p]),
@@ -282,6 +298,7 @@ _SIGS = {
     "tsdrgpu_pipeline_set_autogain": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "tsdrgpu_pipeline_set_contrast": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_pipeline_set_denoise": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "tsdrgpu_pipeline_set_deblur": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_pipeline_set_stack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_pipeline_set_channel": (C.c_int, [C.c_void_p, C.POINTER(ChannelSpec)]),
     "tsdrgpu_pipeline_set_spectrum": (C.c_int, [C.c_void_p, C.POINTER(WelchSpec)]),

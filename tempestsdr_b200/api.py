@@ -151,6 +151,18 @@ class Context:
                                        frames.numel() // (width * height), h_milli, r, p))
         return out
 
+    def deblur(self, frames: torch.Tensor, width: int, height: int, spec: str, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Richardson-Lucy deconvolution along the lines (tsdrgpu.h) of frames.numel() // (width * height) frames back to back,
+        spec "rl:<sigma>[:<I>]"; out must not overlap frames."""
+        mode, sigma_centi, iters = N.deblur_mode(spec)
+        if mode != N.DEBLUR_RL:
+            raise ValueError(f"Context.deblur needs an 'rl:...' spec, not {spec!r}")
+        frames = _f32(frames)
+        out = torch.empty_like(frames) if out is None else out
+        self.chk(self._lib.tsdrgpu_deblur(self._h, self.stream, frames.data_ptr(), out.data_ptr(), width, height,
+                                          frames.numel() // (width * height), sigma_centi, iters))
+        return out
+
     # ------------------------------------------------------------------ a19, a20
     def fft_getrealsize(self, size: int) -> int:
         return self._lib.tsdrgpu_fft_getrealsize(size)
@@ -491,6 +503,11 @@ class PostProcessor:
         """"off" (the default) or "nlm:<h>[:<R>:<P>]" (non-local means of the delivered frames, ahead of CLAHE, tsdrgpu.h) for
         the following runs; kept across reset."""
         self.ctx.chk(self.ctx._lib.tsdrgpu_framestage_set_denoise(self._h, *N.denoise_mode(spec)))
+
+    def set_deblur(self, spec: str) -> None:
+        """"off" (the default) or "rl:<sigma>[:<I>]" (Richardson-Lucy deconvolution along the lines of the delivered frames,
+        after the stack and ahead of NLM and CLAHE, tsdrgpu.h) for the following runs; kept across reset."""
+        self.ctx.chk(self.ctx._lib.tsdrgpu_framestage_set_deblur(self._h, *N.deblur_mode(spec)))
 
     def set_stack(self, spec: str) -> None:
         """"off" (the default), "align:<N>[:<rx>x<ry>]" (drift-registered averaging of the delivered frames, ahead of NLM and

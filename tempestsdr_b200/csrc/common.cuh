@@ -139,14 +139,16 @@ struct StackState {
 int stack_reserve(tsdrgpu_ctx_t *ctx, StackState *st, int nframes, int w, int h);
 int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h);
 int stack_set(StackState *st, int mode, int depth, int rx, int ry);
-// enhance.cu: stack, then NLM, then CLAHE on delivered frames, modes and parameters as the frame stage's setters take them
+// enhance.cu: stack, deblur, NLM, then CLAHE on delivered frames, modes and parameters as the frame stage's setters take them
 struct EnhanceState {
 	int contrast, clip_centi, tx, ty;            // TSDRGPU_CONTRAST_* and its parameters
 	int denoise, h_milli, r, p;                  // TSDRGPU_DENOISE_* and its parameters (R, P)
+	int deblur, sigma_centi, iters;              // TSDRGPU_DEBLUR_* and its parameters (sigma, I)
 	DeviceBuf<unsigned> d_clahe;                 // CLAHE histograms / LUTs of one pass
 	DeviceBuf<float> d_nlm;                      // NLM output of a batch
 	StackState stack;                            // the stack's mode and state
 	DeviceBuf<float> d_stack;                    // stack output of a batch
+	DeviceBuf<float> d_deblur;                   // deblur output of a batch
 };
 // framestage.cu, for the pipeline: restart != 0 restarts the stack; h_records_pinned (may be NULL) receives the stack records of
 // the next run, copied on the stream its output becomes valid on

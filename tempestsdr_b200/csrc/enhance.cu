@@ -1,6 +1,6 @@
 // enhance.cu -- the opt-in steps on the frames the frame stage delivers, beyond the reference (definitions in tsdrgpu.h):
-// drift-registered averaging (stack.cu), non-local means denoising (fs_nlm), then contrast-limited adaptive histogram
-// equalisation (fs_clahe_*).  None feeds back into the frame stage.  Built with -fmad=false like the frame stage, so every output bit follows the definitions.
+// drift-registered averaging (stack.cu), Richardson-Lucy deconvolution along the lines (fs_deblur), non-local means denoising
+// (fs_nlm), then contrast-limited adaptive histogram equalisation (fs_clahe_*).  None feeds back into the frame stage.  Built with -fmad=false like the frame stage, so every output bit follows the definitions.
 #include "common.cuh"
 #include "host_plan.h"
 
@@ -310,7 +310,163 @@ __global__ void __launch_bounds__(NL_TW * NL_BY) fs_nlm(const float *__restrict_
 	}
 }
 
+// ---------------------------------------------------------------- Richardson-Lucy deconvolution along the lines (beyond the reference; the definition is in tsdrgpu.h)
+// A CTA holds up to DB_SPAN pixels of content in shared memory: either several whole lines (lines of at most DB_SPAN pixels,
+// stored R apart so the zeros between them stand for "outside the line"), or one segment of a longer line with a halo of 2 R I
+// pixels on each side, clamped to the line.  It runs all I iterations there and writes the lines or the segment once.  Four
+// planes: d, u, q and rn, with rn = 0 where m = 0, so every plane is 0 wherever m is (u_0 = d = 0 there, q = d / max(b, eps) = 0,
+// u (B(q) rn) = 0): the masked correlation is then a plain one over zeros, and the gaps and pads need no test.  Each thread
+// computes four adjacent outputs from one float4-aligned register window of the plane it correlates.  Where a segment is cut,
+// the plane is correct one R further in after each correlation, so each pass computes only the range the output still needs.
+constexpr int DB_SPAN = 6144;                         // content pixels per CTA: 4 planes of 24 KB, two CTAs per SM
+constexpr int DB_THREADS = 256;
+struct DbTaps { float k[2 * TSDRGPU_DEBLUR_MAX_R + 1]; };
+
+// plane pitch in floats: pads of P = R rounded up to 4 (zeros) around DB_SPAN of content
+__host__ __device__ constexpr int db_pad(int R) { return (R + 3) & ~3; }
+__host__ __device__ constexpr int db_pitch(int R) { return db_pad(R) + DB_SPAN + db_pad(R) + 4; }
+
+// sum_j k_j a(x + t + j), j from -R to R left to right, for t = 0..3; `a` points at content position x (16-byte aligned)
+template <int R, int P>
+__device__ __forceinline__ float4 db_corr4(const float *a, const DbTaps &tp) {
+	constexpr int NW = 2 * P / 4 + 1;
+	float v[4 * NW];
+	const float4 *a4 = reinterpret_cast<const float4 *>(a - P);
+#pragma unroll
+	for (int i = 0; i < NW; i++) { const float4 f = a4[i]; v[4 * i] = f.x; v[4 * i + 1] = f.y; v[4 * i + 2] = f.z; v[4 * i + 3] = f.w; }
+	float s[4];
+#pragma unroll
+	for (int t = 0; t < 4; t++) {
+		s[t] = __fmul_rn(tp.k[0], v[P + t - R]);
+#pragma unroll
+		for (int j = 1; j <= 2 * R; j++) s[t] = __fadd_rn(s[t], __fmul_rn(tp.k[j], v[P + t - R + j]));
+	}
+	return make_float4(s[0], s[1], s[2], s[3]);
+}
+
+// grid.x = CTAs.  Whole lines (seg == 0): CTA c takes lines [c L, min((c + 1) L, lines)) of w pixels, stored at content
+// position l (w + R).  Segments (seg > 0): CTA c takes segment c % segs of line c / segs, [s0, s0 + seg), loaded with its halo.
+template <int R>
+__global__ void __launch_bounds__(DB_THREADS, 2) fs_deblur(const float *__restrict__ in, float *__restrict__ out, int w,
+                                                          long long lines, int L, int seg, int segs, int iters, DbTaps tp) {
+	constexpr int P = db_pad(R), PITCH = db_pitch(R);
+	extern __shared__ __align__(16) float db_smem[];
+	float *sd = db_smem, *su = sd + PITCH, *sq = su + PITCH, *srn = sq + PITCH;
+	long long g0;                                        // first global pixel of the content
+	int span, cutl = 0, cutr = 0, nl = 1, s_out0 = 0, n_out;
+	if (seg == 0) {
+		const long long l0 = (long long) blockIdx.x * L;
+		nl = (int) ((lines - l0 < L) ? lines - l0 : L);
+		g0 = l0 * w;
+		span = nl * (w + R) - R;
+		n_out = nl * w;
+	} else {
+		const long long line = blockIdx.x / (unsigned) segs;
+		const int s0 = (int) (blockIdx.x % (unsigned) segs) * seg, s1 = min(s0 + seg, w), halo = 2 * R * iters;
+		const int a = max(s0 - halo, 0), b = min(s1 + halo, w);
+		cutl = a > 0; cutr = b < w;
+		g0 = line * w + a;
+		span = b - a;
+		s_out0 = s0 - a;
+		n_out = s1 - s0;
+	}
+	const int span4 = (span + 3) & ~3;
+	const float *src = in + g0;
+	// load: d, u = d, m into sq (B(m) gives rn), zeros in the pads and gaps
+	for (int p = threadIdx.x; p < PITCH; p += DB_THREADS) {
+		const int x = p - P;
+		float v = 0.0f, mv = 0.0f;
+		if (x >= 0 && x < span) {
+			const int l = x / (w + R), c = x - l * (w + R);
+			if (c < w) {
+				const float f = __ldg(src + (long long) l * w + c);
+				if (px_valid(f)) { mv = 1.0f; v = f > 0.0f ? fminf(f, 1.0f) : 0.0f; }
+			}
+		}
+		sd[p] = v; su[p] = v; sq[p] = mv; srn[p] = 0.0f;
+	}
+	__syncthreads();
+	for (int g = threadIdx.x; g < span4 / 4; g += DB_THREADS) {
+		const int x = 4 * g;
+		const float4 b = db_corr4<R, P>(sq + P + x, tp), m = *reinterpret_cast<const float4 *>(sq + P + x);
+		float4 r;
+		r.x = m.x != 0.0f ? __fdiv_rn(1.0f, b.x) : 0.0f;
+		r.y = m.y != 0.0f ? __fdiv_rn(1.0f, b.y) : 0.0f;
+		r.z = m.z != 0.0f ? __fdiv_rn(1.0f, b.z) : 0.0f;
+		r.w = m.w != 0.0f ? __fdiv_rn(1.0f, b.w) : 0.0f;
+		*reinterpret_cast<float4 *>(srn + P + x) = r;
+	}
+	__syncthreads();
+	const float eps = TSDRGPU_DEBLUR_EPS;
+	for (int it = 0, k = 1; it < iters; it++, k += 2) {
+		// pass 1: q = d / max(B(u) rn, eps), on the range correct after k correlations
+		int lo = cutl ? (k * R) & ~3 : 0, hi = cutr ? min((span - k * R + 3) & ~3, span4) : span4;
+		for (int g = lo / 4 + threadIdx.x; g < hi / 4; g += DB_THREADS) {
+			const int x = 4 * g;
+			const float4 b = db_corr4<R, P>(su + P + x, tp);
+			const float4 rn = *reinterpret_cast<const float4 *>(srn + P + x), d = *reinterpret_cast<const float4 *>(sd + P + x);
+			float4 q;
+			q.x = __fdiv_rn(d.x, fmaxf(__fmul_rn(b.x, rn.x), eps));
+			q.y = __fdiv_rn(d.y, fmaxf(__fmul_rn(b.y, rn.y), eps));
+			q.z = __fdiv_rn(d.z, fmaxf(__fmul_rn(b.z, rn.z), eps));
+			q.w = __fdiv_rn(d.w, fmaxf(__fmul_rn(b.w, rn.w), eps));
+			*reinterpret_cast<float4 *>(sq + P + x) = q;
+		}
+		__syncthreads();
+		// pass 2: u = u (B(q) rn), in place (each output reads only its own u)
+		lo = cutl ? ((k + 1) * R) & ~3 : 0; hi = cutr ? min((span - (k + 1) * R + 3) & ~3, span4) : span4;
+		for (int g = lo / 4 + threadIdx.x; g < hi / 4; g += DB_THREADS) {
+			const int x = 4 * g;
+			const float4 c = db_corr4<R, P>(sq + P + x, tp);
+			const float4 rn = *reinterpret_cast<const float4 *>(srn + P + x);
+			float4 u = *reinterpret_cast<const float4 *>(su + P + x);
+			u.x = __fmul_rn(u.x, __fmul_rn(c.x, rn.x));
+			u.y = __fmul_rn(u.y, __fmul_rn(c.y, rn.y));
+			u.z = __fmul_rn(u.z, __fmul_rn(c.z, rn.z));
+			u.w = __fmul_rn(u.w, __fmul_rn(c.w, rn.w));
+			*reinterpret_cast<float4 *>(su + P + x) = u;
+		}
+		__syncthreads();
+	}
+	// output: the lines or the segment, at any 4-byte phase
+	const float *osrc = src + s_out0;
+	float *dst = out + g0 + s_out0;
+	for (int e = threadIdx.x; e < n_out; e += DB_THREADS) {
+		const int l = e / w, c = e - l * w;
+		const float v = __ldg(osrc + e);
+		dst[e] = px_valid(v) ? fminf(su[P + s_out0 + l * (w + R) + c], 1.0f) : v;
+	}
+}
+
 }  // namespace
+
+// deblur of nframes frames of w x h, in -> out (no overlap), on `stream`
+static int fs_deblur_batch(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h,
+                           int sigma_centi, int iters) {
+	DbTaps tp = {};
+	int R = 0;
+	if (tsdrgpu_deblur_taps(sigma_centi, tp.k, &R) != TSDRGPU_OK) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "deblur sigma", cudaSuccess, __FILE__, __LINE__);
+	const long long lines = (long long) nframes * h;
+	int L = 0, seg = 0, segs = 0;
+	long long ctas;
+	if (w <= DB_SPAN) {                                  // whole lines, R apart
+		L = (DB_SPAN + R) / (w + R);
+		ctas = (lines + L - 1) / L;
+	} else {                                             // segments with a halo of 2 R I on each side
+		seg = DB_SPAN - 4 * R * iters;
+		segs = (w + seg - 1) / seg;
+		ctas = lines * segs;
+	}
+	ARG_TRY(ctx, ctas <= 0x7fffffffLL);
+	using K = void (*)(const float *, float *, int, long long, int, int, int, int, DbTaps);
+	static const K kernels[TSDRGPU_DEBLUR_MAX_R] = {fs_deblur<1>, fs_deblur<2>, fs_deblur<3>, fs_deblur<4>, fs_deblur<5>, fs_deblur<6>,
+	                                                fs_deblur<7>, fs_deblur<8>, fs_deblur<9>, fs_deblur<10>, fs_deblur<11>, fs_deblur<12>};
+	const K kern = kernels[R - 1];
+	const size_t smem = sizeof(float) * 4 * (size_t) db_pitch(R);
+	CU_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+	KL(ctx, "fs_deblur", stream, kern<<<(unsigned) ctas, DB_THREADS, smem, stream>>>(in, out, w, lines, L, seg, segs, iters, tp));
+	return TSDRGPU_OK;
+}
 
 // CLAHE: effective tile grid, frames per pass and the words one pass of the histogram buffer needs
 struct ChGeom { int tx, ty, fpp; size_t words; };
@@ -387,6 +543,7 @@ int enhance_reserve(tsdrgpu_ctx_t *ctx, EnhanceState *st, int nframes, int w, in
 		if (rc) return rc;
 		if (st->d_stack.cap < nlm) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, st->d_stack.assign(nlm)); }
 	}
+	if (st->deblur == TSDRGPU_DEBLUR_RL && st->d_deblur.cap < nlm) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, st->d_deblur.assign(nlm)); }
 	if (st->denoise == TSDRGPU_DENOISE_NLM && st->d_nlm.cap < nlm) { CU_TRY(ctx, cudaDeviceSynchronize()); CU_TRY(ctx, st->d_nlm.assign(nlm)); }
 	if (st->contrast != TSDRGPU_CONTRAST_CLAHE) return TSDRGPU_OK;
 	const size_t words = ch_geom(st, nframes, w, h).words;
@@ -394,9 +551,9 @@ int enhance_reserve(tsdrgpu_ctx_t *ctx, EnhanceState *st, int nframes, int w, in
 	return TSDRGPU_OK;
 }
 
-// The stack, NLM, then CLAHE, in place on nframes frames of w x h, on `stream`.  Neither the stack nor NLM can run in place: the
-// stack writes d_stack, NLM writes d_nlm (or, after the stack, the frames themselves), and CLAHE or one copy brings the frames
-// back.  Only `stream` ever touches these buffers and the stack's state: the frame stage passes the stream its output becomes
+// The stack, deblur, NLM, then CLAHE, in place on nframes frames of w x h, on `stream`.  None of the first three can run in place:
+// each writes its own buffer (d_stack, d_deblur, d_nlm) when it reads the frames themselves, and the frames when it reads a buffer,
+// and CLAHE or one copy brings the frames back.  Only `stream` ever touches these buffers and the stack's state: the frame stage passes the stream its output becomes
 // valid on, and in overlap mode its main stream is already filling d_t1 and the other phase's T2 with the next batch, so neither
 // can be borrowed.
 int enhance_run(tsdrgpu_ctx_t *ctx, EnhanceState *st, cudaStream_t stream, float *d_frames, int nframes, int w, int h) {
@@ -407,6 +564,11 @@ int enhance_run(tsdrgpu_ctx_t *ctx, EnhanceState *st, cudaStream_t stream, float
 	if (stack) {
 		if ((rc = stack_run(ctx, &st->stack, stream, cur, st->d_stack.ptr, nframes, w, h))) return rc;
 		cur = st->d_stack.ptr;
+	}
+	if (st->deblur == TSDRGPU_DEBLUR_RL) {
+		float *dst = (cur == d_frames) ? st->d_deblur.ptr : d_frames;
+		if ((rc = fs_deblur_batch(ctx, stream, cur, dst, nframes, w, h, st->sigma_centi, st->iters))) return rc;
+		cur = dst;
 	}
 	if (nlm) {
 		float *dst = (cur == d_frames) ? st->d_nlm.ptr : d_frames;
@@ -445,6 +607,20 @@ int tsdrgpu_nlm(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_in, float *d_o
 	ARG_TRY(ctx, (uintptr_t) d_out >= (uintptr_t) d_in + bytes || (uintptr_t) d_in >= (uintptr_t) d_out + bytes);
 	cudaStream_t stream = (cudaStream_t) stream_;
 	int rc = fs_nlm_batch(ctx, stream, d_in, d_out, nframes, w, h, h_milli, r, p);
+	if (rc == TSDRGPU_OK) CU_TRY(ctx, cudaStreamSynchronize(stream));
+	return rc;
+}
+
+int tsdrgpu_deblur(tsdrgpu_ctx_t *ctx, void *stream_, const float *d_in, float *d_out, int w, int h, int nframes, int sigma_centi,
+                   int iterations) {
+	BIND(ctx);
+	if (nframes == 0) return TSDRGPU_OK;
+	ARG_TRY(ctx, d_in && d_out && nframes > 0 && w > 0 && h > 0 && (size_t) w * h <= TSDRGPU_MAX_FRAME_PIXELS);
+	ARG_TRY(ctx, ((((uintptr_t) d_in) | ((uintptr_t) d_out)) & 3) == 0 && deblur_ok(TSDRGPU_DEBLUR_RL, sigma_centi, iterations));
+	const uintptr_t bytes = (uintptr_t) sizeof(float) * w * h * nframes;
+	ARG_TRY(ctx, (uintptr_t) d_out >= (uintptr_t) d_in + bytes || (uintptr_t) d_in >= (uintptr_t) d_out + bytes);
+	cudaStream_t stream = (cudaStream_t) stream_;
+	int rc = fs_deblur_batch(ctx, stream, d_in, d_out, nframes, w, h, sigma_centi, iterations);
 	if (rc == TSDRGPU_OK) CU_TRY(ctx, cudaStreamSynchronize(stream));
 	return rc;
 }

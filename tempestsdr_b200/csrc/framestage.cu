@@ -1516,7 +1516,7 @@ struct tsdrgpu_framestage {
 	int batch_cap;                               // frames every per-batch buffer holds (0 until all of them are allocated)
 	int ag_mode, ag_ppm;                         // tsdrgpu_framestage_set_autogain (kept across reset)
 	DeviceBuf<unsigned> d_sel_hist; DeviceBuf<SelState> d_sel; DeviceBuf<float2> d_levels;     // clip-mode selection, batch_cap frames
-	EnhanceState enh;                            // tsdrgpu_framestage_set_contrast / _set_denoise / _set_stack (kept across reset)
+	EnhanceState enh;                            // tsdrgpu_framestage_set_contrast / _set_denoise / _set_stack / _set_deblur (kept across reset)
 	tsdrgpu_stack_record_t *h_stack_next;        // framestage_stack_next: where the next run's stack records go
 	DeviceBuf<tsdrgpu_frame_result_t> d_results[2];
 	DeviceBuf<double> d_chain;
@@ -1704,6 +1704,14 @@ int tsdrgpu_framestage_set_denoise(tsdrgpu_framestage_t *fs, int mode, int h_mil
 	ARG_TRY(fs->ctx, denoise_ok(mode, h_milli, r, p));
 	fs->enh.denoise = mode;
 	if (mode == TSDRGPU_DENOISE_NLM) { fs->enh.h_milli = h_milli; fs->enh.r = r; fs->enh.p = p; }
+	return TSDRGPU_OK;
+}
+
+int tsdrgpu_framestage_set_deblur(tsdrgpu_framestage_t *fs, int mode, int sigma_centi, int iterations) {
+	ARG_TRY((tsdrgpu_ctx_t *) NULL, fs != NULL);
+	ARG_TRY(fs->ctx, deblur_ok(mode, sigma_centi, iterations));
+	fs->enh.deblur = mode;
+	if (mode == TSDRGPU_DEBLUR_RL) { fs->enh.sigma_centi = sigma_centi; fs->enh.iters = iterations; }
 	return TSDRGPU_OK;
 }
 
@@ -1906,7 +1914,7 @@ static int framestage_run_impl(tsdrgpu_framestage_t *fs, void *stream_, const fl
 			KL(ctx, "fs_results_autogain", stream, fs_results_autogain<<<1, 256, 0, stream>>>(nframes, fs->d_params.ptr, fs->d_state.ptr, d_results));
 		}
 	}
-	// NLM, then CLAHE, on the frames as delivered, after every branch's last step; nothing either does feeds back
+	// the stack, deblur, NLM, then CLAHE, on the frames as delivered, after every branch's last step; nothing either does feeds back
 	if ((rc = enhance_run(ctx, &fs->enh, tail, d_out, nframes, w, h))) return rc;
 	if (fs->h_stack_next && fs->enh.stack.mode != TSDRGPU_STACK_OFF)
 		CU_TRY(ctx, cudaMemcpyAsync(fs->h_stack_next, fs->enh.stack.d_rec.ptr, sizeof(tsdrgpu_stack_record_t) * nframes, cudaMemcpyDeviceToHost, tail));

@@ -196,7 +196,7 @@ uint32_t tsdrgpu_spectrum_k(const tsdrgpu_welch_t *spec, uint32_t fs) {
 	return k > 0 ? (uint32_t) k : 1u;
 }
 
-/* ---- auto-gain, contrast and denoise options (definitions in tsdrgpu.h) */
+/* ---- auto-gain, contrast, denoise, stack and deblur options (definitions in tsdrgpu.h) */
 int autogain_ok(int mode, int ppm) {
 	return (mode == TSDRGPU_AG_MINMAX || mode == TSDRGPU_AG_CLIP) && ppm >= 0 && ppm <= TSDRGPU_AG_MAX_PPM;
 }
@@ -214,6 +214,11 @@ int denoise_ok(int mode, int h_milli, int r, int p) {
 int stack_ok(int mode, int depth, int rx, int ry) {
 	return mode == TSDRGPU_STACK_OFF || ((mode == TSDRGPU_STACK_ALIGN || mode == TSDRGPU_STACK_ADAPT) && depth >= TSDRGPU_STACK_MIN_N &&
 	       depth <= TSDRGPU_STACK_MAX_N && rx >= 1 && rx <= TSDRGPU_STACK_MAX_RX && ry >= 0 && ry <= TSDRGPU_STACK_MAX_RY);
+}
+
+int deblur_ok(int mode, int sigma_centi, int iterations) {
+	return mode == TSDRGPU_DEBLUR_OFF || (mode == TSDRGPU_DEBLUR_RL && sigma_centi >= TSDRGPU_DEBLUR_MIN_SIGMA &&
+	       sigma_centi <= TSDRGPU_DEBLUR_MAX_SIGMA && iterations >= 1 && iterations <= TSDRGPU_DEBLUR_MAX_ITER);
 }
 
 /* one to six decimal digits -> their value, *c moved past them; -1 for none or more than six */
@@ -276,6 +281,41 @@ int tsdrgpu_stack_parse(const char *spec, int *mode, int *depth, int *rx, int *r
 	if (!on) m = TSDRGPU_STACK_OFF;
 	if (!stack_ok(m, v[0], v[1], v[2])) return TSDRGPU_EINVAL;
 	*mode = m; *depth = v[0]; *rx = v[1]; *ry = v[2];
+	return TSDRGPU_OK;
+}
+
+/* its own small rule, as it takes one optional value: "rl:<sigma>[:<I>]", sigma with at most two fraction digits */
+int tsdrgpu_deblur_parse(const char *spec, int *mode, int *sigma_centi, int *iterations) {
+	if (!spec || !mode || !sigma_centi || !iterations) return TSDRGPU_EINVAL;
+	if (strcmp(spec, "off") == 0) { *mode = TSDRGPU_DEBLUR_OFF; *sigma_centi = 0; *iterations = 0; return TSDRGPU_OK; }
+	if (strncmp(spec, "rl:", 3) != 0) return TSDRGPU_EINVAL;
+	const char *c = spec + 3;
+	int s = option_digits(&c), it = 20;
+	if (s < 0) return TSDRGPU_EINVAL;
+	s *= 100;
+	if (*c == '.') {
+		const char *f = ++c;
+		int frac = option_digits(&c);
+		const int nd = (int) (c - f);
+		if (frac < 0 || nd > 2) return TSDRGPU_EINVAL;
+		s += nd == 1 ? 10 * frac : frac;
+	}
+	if (*c == ':') { c++; if ((it = option_digits(&c)) < 0) return TSDRGPU_EINVAL; }
+	if (*c || !deblur_ok(TSDRGPU_DEBLUR_RL, s, it)) return TSDRGPU_EINVAL;
+	*mode = TSDRGPU_DEBLUR_RL; *sigma_centi = s; *iterations = it;
+	return TSDRGPU_OK;
+}
+
+/* the deblur taps (definition in tsdrgpu.h) */
+int tsdrgpu_deblur_taps(int sigma_centi, float *taps, int *R) {
+	if (!deblur_ok(TSDRGPU_DEBLUR_RL, sigma_centi, 1)) return TSDRGPU_EINVAL;
+	const int r = (3 * sigma_centi + 99) / 100;
+	if (R) *R = r;
+	if (!taps) return TSDRGPU_OK;
+	const double s = sigma_centi / 100.0;
+	double e[2 * TSDRGPU_DEBLUR_MAX_R + 1], sum = 0.0;
+	for (int j = -r; j <= r; j++) { e[j + r] = exp(-(double) (j * j) / (2.0 * s * s)); sum += e[j + r]; }
+	for (int j = 0; j <= 2 * r; j++) taps[j] = (float) (e[j] / sum);
 	return TSDRGPU_OK;
 }
 

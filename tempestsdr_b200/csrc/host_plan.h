@@ -7,11 +7,12 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
-/* internal: 1 when a mode and its parameters are in tsdrgpu.h's ranges (contrast, denoise and stack ignore them when off), else 0 */
+/* internal: 1 when a mode and its parameters are in tsdrgpu.h's ranges (contrast, denoise, stack and deblur ignore them when off), else 0 */
 int autogain_ok(int mode, int ppm);
 int contrast_ok(int mode, int clip_centi, int tx, int ty);
 int denoise_ok(int mode, int h_milli, int r, int p);
 int stack_ok(int mode, int depth, int rx, int ry);
+int deblur_ok(int mode, int sigma_centi, int iterations);
 #ifdef __cplusplus
 }
 #endif

@@ -63,6 +63,7 @@ struct Settings {
 	int ct_mode = TSDRGPU_CONTRAST_OFF, ct_clip = 200, ct_tx = 8, ct_ty = 8;
 	int nl_mode = TSDRGPU_DENOISE_OFF, nl_h = 100, nl_r = 5, nl_p = 1;
 	int st_mode = TSDRGPU_STACK_OFF, st_depth = 32, st_rx = 8, st_ry = 2;
+	int db_mode = TSDRGPU_DEBLUR_OFF, db_sigma = 100, db_iters = 20;
 	int stack_restart = 0;                             // tsdr_sync: the stack restarts at the next frame-stage batch
 	tsdrgpu_channel_t cf_spec = {};                    // taps == 0: off; applied per process()
 	tsdrgpu_welch_t sp_spec = {};                      // n == 0: off; applied per process()
@@ -502,6 +503,7 @@ static int drain_frames(tsdrgpu_pipeline *p, const Settings &s) {
 		if ((rc = tsdrgpu_framestage_set_contrast(p->fs, s.ct_mode, s.ct_clip, s.ct_tx, s.ct_ty))) return rc;
 		if ((rc = tsdrgpu_framestage_set_denoise(p->fs, s.nl_mode, s.nl_h, s.nl_r, s.nl_p))) return rc;
 		if ((rc = tsdrgpu_framestage_set_stack(p->fs, s.st_mode, s.st_depth, s.st_rx, s.st_ry))) return rc;
+		if ((rc = tsdrgpu_framestage_set_deblur(p->fs, s.db_mode, s.db_sigma, s.db_iters))) return rc;
 		const bool stack_on = s.st_mode != TSDRGPU_STACK_OFF;
 		if ((rc = framestage_stack_next(p->fs, take_request(p, p->set.stack_restart), stack_on ? p->h_stack[slot].ptr : NULL))) return rc;
 		if ((rc = tsdrgpu_framestage_run_async(p->fs, p->s_main, p->d_pix.ptr + p->pix_read, nf, w, h, s.motionblur,
@@ -787,6 +789,12 @@ int tsdrgpu_pipeline_set_stack(tsdrgpu_pipeline_t *p, int mode, int depth, int r
 	return update(p, stack_ok(mode, depth, rx, ry), [&](Settings &s) {
 		if (mode != TSDRGPU_STACK_OFF) { s.st_depth = depth; s.st_rx = rx; s.st_ry = ry; }
 		s.st_mode = mode;
+	});
+}
+int tsdrgpu_pipeline_set_deblur(tsdrgpu_pipeline_t *p, int mode, int sigma_centi, int iterations) {
+	return update(p, deblur_ok(mode, sigma_centi, iterations), [&](Settings &s) {
+		if (mode == TSDRGPU_DEBLUR_RL) { s.db_sigma = sigma_centi; s.db_iters = iterations; }
+		s.db_mode = mode;
 	});
 }
 int tsdrgpu_pipeline_sync(tsdrgpu_pipeline_t *p, int pixels) { return update(p, true, [&](Settings &s) { s.syncoffset += pixels; s.stack_restart = 1; }); }

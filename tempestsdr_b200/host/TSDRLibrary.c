@@ -419,6 +419,17 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 			goto end;
 		}
 	}
+	/* TSDR_DEBLUR=rl:<sigma>[:<I>]: Richardson-Lucy deconvolution along the lines of the delivered frames, after the stack and
+	 * ahead of NLM and CLAHE (tsdrgpu.h).  Unset or "off": none */
+	int db_mode = TSDRGPU_DEBLUR_OFF, db_sigma = 0, db_iters = 0;
+	{
+		const char *db = getenv("TSDR_DEBLUR");
+		if (db && tsdrgpu_deblur_parse(db, &db_mode, &db_sigma, &db_iters) != TSDRGPU_OK) {
+			status = fail(t, "TSDR_DEBLUR must be \"off\", \"rl:<sigma>\" or \"rl:<sigma>:<I>\" with sigma in [0.25, 4] and I in [1, 64]",
+			              TSDR_INVALID_PARAMETER_VALUE);
+			goto end;
+		}
+	}
 
 	/* TSDR_CUDA_DEVICES="0,1,2,3": superbandwidth mode records one hop per listed GPU and shards the stitch over them
 	 * (tsdrgpu_pipeline_set_superb_devices); the first entry is the device everything else runs on.  TSDR_CUDA_DEVICE=n: one GPU. */
@@ -472,6 +483,7 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 			if (ct_mode != TSDRGPU_CONTRAST_OFF) tsdrgpu_pipeline_set_contrast(np, ct_mode, ct_clip, ct_tx, ct_ty);
 			if (nl_mode != TSDRGPU_DENOISE_OFF) tsdrgpu_pipeline_set_denoise(np, nl_mode, nl_h, nl_r, nl_p);
 			if (st_mode != TSDRGPU_STACK_OFF) tsdrgpu_pipeline_set_stack(np, st_mode, st_depth, st_rx, st_ry);
+			if (db_mode != TSDRGPU_DEBLUR_OFF) tsdrgpu_pipeline_set_deblur(np, db_mode, db_sigma, db_iters);
 			if (channel.taps != 0) tsdrgpu_pipeline_set_channel(np, &channel);
 			if (spectrum.n != 0) tsdrgpu_pipeline_set_spectrum(np, &spectrum);
 		}

@@ -26,7 +26,7 @@ class Pipeline:
                  on_frame: Optional[Callable] = None, on_value: Optional[Callable] = None, on_plot: Optional[Callable] = None,
                  on_retune: Optional[Callable] = None, resampler: str = "box", autogain: str = "minmax",
                  contrast: str = "off", channel: str = "off", denoise: str = "off", spectrum: str = "off",
-                 stack: str = "off"):
+                 stack: str = "off", deblur: str = "off"):
         self._lib = N.lib()
         ctx = C.c_void_p()
         N.check(self._lib.tsdrgpu_create(C.byref(ctx), device))
@@ -77,6 +77,8 @@ class Pipeline:
             self.set_spectrum(spectrum)
         if stack != "off":
             self.set_stack(stack)
+        if deblur != "off":
+            self.set_deblur(deblur)
         if on_retune:
             def _retune(off, _):
                 try:
@@ -152,6 +154,11 @@ class Pipeline:
         frame-stage batch on.  While it is on, on_value also receives (101, drift in px/frame,
         offset mod W H) beside every auto-gain report; sync() restarts the average."""
         N.check(self._lib.tsdrgpu_pipeline_set_stack(self._h, *N.stack_mode(spec)), self._ctx)
+
+    def set_deblur(self, spec: str) -> None:
+        """"off" (the default) or "rl:<sigma>[:<I>]" (Richardson-Lucy deconvolution along the lines of the delivered frames,
+        after the stack and ahead of NLM and CLAHE, tsdrgpu.h) from the next frame-stage batch on."""
+        N.check(self._lib.tsdrgpu_pipeline_set_deblur(self._h, *N.deblur_mode(spec)), self._ctx)
 
     def set_channel(self, spec: str) -> None:
         """"off" (the default) or "pass:<lo>:<hi>[,stop:<a>:<b>]...[,taps:<T>]" (the channel filter on the IQ stream before
