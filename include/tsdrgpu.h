@@ -139,7 +139,9 @@ TSDRGPU_API int  tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream, con
 
 /* One-shot: the NEXT tsdrgpu_resampler_run with IQ input also writes |x| of every input sample to d_mag (one float per
  * sample, blocks back to back like d_in) -- am_demod's output for the frame-rate detector (TSDRLibrary.c:286-292 feeds both
- * consumers from one demodulated buffer) without a second pass over the IQ. */
+ * consumers from one demodulated buffer) without a second pass over the IQ.  A refused run leaves it armed, as it leaves
+ * the state: a run refused for asking magnitudes of magnitude input or of the nearest-neighbour mode is refused again
+ * until the caller disarms it (d_mag = NULL). */
 TSDRGPU_API int  tsdrgpu_resampler_set_mag_out(tsdrgpu_resampler_t *r, float *d_mag);
 
 /* ---------------------------------------------------------------------------- a2-  channel filter (beyond the reference)

@@ -441,8 +441,11 @@ class Resampler:
         if out is None:
             out = torch.empty(max(int(need), 1), dtype=torch.float32, device=x.device)
         n_out = C.c_uint64(0)
-        self.ctx.chk(self.ctx._lib.tsdrgpu_resampler_run(self._h, self.ctx.stream, _f32(x).data_ptr(), int(in_is_iq), p, u, n,
-                                                         upsample_by, downsample_by, int(nearest), out.data_ptr(), out.numel(), C.byref(n_out)))
+        rc = self.ctx._lib.tsdrgpu_resampler_run(self._h, self.ctx.stream, _f32(x).data_ptr(), int(in_is_iq), p, u, n,
+                                                 upsample_by, downsample_by, int(nearest), out.data_ptr(), out.numel(), C.byref(n_out))
+        if rc != N.OK and mag_out is not None:       # a refused run leaves mag_out armed: disarm it, it belongs to this call only
+            self.ctx._lib.tsdrgpu_resampler_set_mag_out(self._h, None)
+        self.ctx.chk(rc)
         return out[: n_out.value]
 
 

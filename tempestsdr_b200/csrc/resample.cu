@@ -688,6 +688,8 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 	const bool sinc = r->kernel == TSDRGPU_RS_SINC && !nearest;
 	if (sinc && !(ratio >= TSDRGPU_SINC_MIN_RATIO))
 		return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "the sinc resampler needs upsample_by/downsample_by >= 1/16", cudaSuccess, __FILE__, __LINE__);
+	// A refused call changes nothing: not the state, not the descriptor ring, not the armed magnitude output.
+	if (r->d_mag_next && (!in_is_iq || nearest)) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "magnitude output needs IQ input and the box resampler", cudaSuccess, __FILE__, __LINE__);
 	const unsigned sinc_pt = sinc ? sinc_pixels_per_tile(ratio) : 0;
 	// descriptor slot: [RsBlock x nblocks][{block, first sample (box) / first pixel (sinc)} x tiles]
 	size_t max_tiles = 0;
@@ -696,7 +698,7 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 		max_tiles += sinc ? (size_t) ((double) size * ratio + 2.0) / sinc_pt + 2 : (size + RS_TILE - 1) / RS_TILE + 1;
 	}
 	const size_t need = sizeof(tsdrgpu_rs_block_t) * nblocks + sizeof(uint2) * (max_tiles + 1);
-	const int slot = r->next; r->next = (r->next + 1) % tsdrgpu_resampler::SLOTS;
+	const int slot = r->next;
 	CU_TRY(ctx, cudaEventSynchronize(r->ev[slot]));
 	if (r->h_desc[slot].cap < need || r->d_desc[slot].cap < need) {
 		const int rc = r->h_desc[slot].assign(ctx, need * 2);
@@ -712,6 +714,7 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 		return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "a block would produce no pixel (the reference asserts here, extbuffer.c:48)", cudaSuccess, __FILE__, __LINE__);
 	if (total > out_capacity)
 		return tsdrgpu_fail(ctx, TSDRGPU_ECAPACITY, "resampler output buffer too small", cudaSuccess, __FILE__, __LINE__);
+	r->next = (slot + 1) % tsdrgpu_resampler::SLOTS;
 	unsigned tiles = 0, max_out = 0;
 	// rs_main4 (four samples per thread) stages every tile's pixels in shared memory: ratios up to 3; beyond that, and on
 	// request (TSDRGPU_RS_V1=1, the cross-check of the tests), the one-sample-per-thread kernel (every geometry the reference
@@ -737,7 +740,6 @@ int tsdrgpu_resampler_run(tsdrgpu_resampler_t *r, void *stream_, const float *d_
 	const uint2 *dp = (const uint2 *) (db + nblocks);
 
 	float *mag = r->d_mag_next; r->d_mag_next = NULL;
-	if (mag && (!in_is_iq || nearest)) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "magnitude output needs IQ input and the box resampler", cudaSuccess, __FILE__, __LINE__);
 	if (sinc) {
 		const double fc = ratio < 1.0 ? ratio : 1.0;
 		if (r->taps_fc != fc) {                           // pageable source: the copy is staged before the call returns
