@@ -700,7 +700,7 @@ TSDRGPU_API int tsdrgpu_superb_residue_ifft_lag(tsdrgpu_ctx_t *ctx, void *stream
  * MAGNITUDE stream (what am_demod makes of superb_run's output, TSDRLibrary.c:271-274).  No host synchronisation, no
  * collective library: flags in peer memory order the phases.  A group object exists once per rank; the windows are tied
  * together either through CUDA IPC handles (one process per GPU: export -> exchange by any means -> connect_ipc) or directly
- * (all ranks in one process: connect_local).  nranks in {2, 4, 8, 16}. */
+ * (all ranks in one process: connect_local).  nranks in {2, 4, 8} (a node has at most eight GPUs). */
 typedef struct tsdrgpu_superb_mgpu tsdrgpu_superb_mgpu_t;
 TSDRGPU_API int  tsdrgpu_superb_mgpu_create(tsdrgpu_ctx_t *ctx, int nranks, int rank, int root, uint32_t max_pairs_per_hop, tsdrgpu_superb_mgpu_t **g);
 TSDRGPU_API void tsdrgpu_superb_mgpu_destroy(tsdrgpu_superb_mgpu_t *g);

@@ -37,7 +37,8 @@
 // other devices of this process (cudaDeviceEnablePeerAccess: the C host library with TSDR_CUDA_DEVICES).
 //
 // Parity: lags exact (same float operations as the one-GPU path up to the transform, first-maximum argmax); samples are
-// tolerance-based like every FFT result here: <= 1e-5 of the peak against superb_ondataready + am_demod (measured ~1e-6).
+// tolerance-based like every FFT result here: within float32 rounding units of a float64 model of this dataflow, and of
+// superb_ondataready + am_demod's model within that plus a pinned deviation (tests/test_superb_sweep.py, DESIGN.md section 6).
 #include "common.cuh"
 #include <math.h>
 #include <stdlib.h>
@@ -154,7 +155,7 @@ __global__ void __launch_bounds__(256) sbm_pull_blocks(PullArgs A, float4 *__res
 struct FinalArgs { Peers peers; size_t off_a, off_r; int H, log2H, rank, root; unsigned n; double eps[4]; };
 template <int H>
 __global__ void __launch_bounds__(256) sbm_final(FinalArgs A) {
-	constexpr int LOG2H = (H == 2) ? 1 : (H == 4) ? 2 : (H == 8) ? 3 : 4;
+	constexpr int LOG2H = (H == 2) ? 1 : (H == 4) ? 2 : 3;
 	__shared__ double2 cfac[LOG2H][H / 2];            // exp(+i pi beta / 2^s (1 + eps_s)), beta < 2^s
 	if (threadIdx.x < LOG2H * (H / 2)) {
 		const int sidx = threadIdx.x / (H / 2), beta = threadIdx.x % (H / 2);
@@ -245,13 +246,19 @@ static int create_handles(tsdrgpu_superb_mgpu *g) {
 	CU_TRY(ctx, g->d_part.assign(8 * TSDRGPU_ARGMAX_PARTS));
 	CU_TRY(ctx, g->d_lag.assign(64));
 	CU_TRY(ctx, cudaMemset(g->d_lag.ptr, 0, 256));
+	// The context's transform scratch, sized now for the largest a stitch runs (the two nd-point difference spectra, nd <= n_max):
+	// growing it synchronises the device, and a rank that does so inside sbm_prepare while a peer on the same device already
+	// spins on a flag of this stitch waits for that peer, which waits for it (found by a second stitch with a larger nd).
+	void *scratch;
+	const int rc = tsdrgpu_scratch(ctx, 0, sizeof(float2) * 2 * n, &scratch);
+	if (rc) return rc;
 	CU_TRY(ctx, cudaDeviceSynchronize());
 	return TSDRGPU_OK;
 }
 
 int tsdrgpu_superb_mgpu_create(tsdrgpu_ctx_t *ctx, int nranks, int rank, int root, uint32_t max_pairs_per_hop, tsdrgpu_superb_mgpu_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
-	ARG_TRY(ctx, (nranks == 2 || nranks == 4 || nranks == 8 || nranks == 16) && rank >= 0 && rank < nranks && root >= 0 && root < nranks && max_pairs_per_hop >= 64);
+	ARG_TRY(ctx, (nranks == 2 || nranks == 4 || nranks == 8) && rank >= 0 && rank < nranks && root >= 0 && root < nranks && max_pairs_per_hop >= 64);
 	tsdrgpu_superb_mgpu *g = new tsdrgpu_superb_mgpu();      // value-initialised: every field not set here starts at zero
 	g->ctx = ctx; g->H = nranks; g->rank = rank; g->root = root;
 	while ((1 << g->log2H) < nranks) g->log2H++;
@@ -368,8 +375,7 @@ static int sbm_prepare(tsdrgpu_superb_mgpu *g, cudaStream_t stream, unsigned N, 
 	switch (g->H) {
 	case 2: preload(sbm_final<2>); break;
 	case 4: preload(sbm_final<4>); break;
-	case 8: preload(sbm_final<8>); break;
-	default: preload(sbm_final<16>); break;
+	default: preload(sbm_final<8>); break;
 	}
 	CU_TRY(ctx, cudaStreamSynchronize(stream));
 	g->prep_n = N; g->prep_nd = nd;
@@ -452,8 +458,7 @@ int tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stream_, const fl
 		switch (H) {
 		case 2: KL(ctx, "sbm_final", stream, sbm_final<2><<<grid, 256, 0, stream>>>(A)); break;
 		case 4: KL(ctx, "sbm_final", stream, sbm_final<4><<<grid, 256, 0, stream>>>(A)); break;
-		case 8: KL(ctx, "sbm_final", stream, sbm_final<8><<<grid, 256, 0, stream>>>(A)); break;
-		default: KL(ctx, "sbm_final", stream, sbm_final<16><<<grid, 256, 0, stream>>>(A)); break;
+		default: KL(ctx, "sbm_final", stream, sbm_final<8><<<grid, 256, 0, stream>>>(A)); break;
 		}
 	}
 	KL(ctx, "sbm_sync", stream, sbm_sync<<<1, 32, 0, stream>>>(g->peers, H, rank, PH_RES, epoch, 1u << g->root, rank == g->root ? all : 0u, (const int *) NULL, g->timeout_cycles));

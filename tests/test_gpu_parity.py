@@ -5,8 +5,6 @@ restatement.  Integer/index results and every float produced by the sample->pixe
 the FFT family is tolerance-based (float32 Stockham vs the reference's float-storage radix-2): the tolerance is
 written next to each check, relative to the peak magnitude of the reference result.
 """
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -521,27 +519,7 @@ def test_superbandwidth(gpu, O):
     _close(sim, want, 8e-6, "one-exchange stitch")
 
 
-@pytest.mark.parametrize("H", [2, 4, 8])
-def test_superbandwidth_one_hop_per_rank_on_one_device(H):
-    """csrc/superb_mgpu.cu (tsdrgpu_superb_mgpu_*) with all H ranks living on THIS GPU (one context and one stream per rank,
-    windows cross-linked by connect_local): the complete product dataflow -- local spectra, lag from rank 0's difference
-    spectrum, all-to-all mix, residue inverse, |.| into the root's slots, interleave -- with its flag synchronisation, on a
-    single device (tests/sbm_one_device.py; a process of its own so that every rank's stream gets a hardware queue of its own)."""
-    import subprocess, sys
-    r = subprocess.run([sys.executable, "-m", "tests.sbm_one_device", str(H)], capture_output=True, text=True, timeout=120,
-                       cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))), env=dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32", TSDRGPU_SBM_TIMEOUT_MS="1500"))
-    assert r.returncode == 0 and "sbm ok" in r.stdout, (r.stdout[-1500:], r.stderr[-1500:])
-
-
-def test_superbandwidth_one_hop_per_rank_at_the_baseline_hop_size():
-    """The same at BASELINE configs[3]'s own size: 4 hops of 10 frames of 25 MS/s IQ (N = 2^21 per hop, a 2^23-point inverse) against
-    superb_ondataready + am_demod of the compiled reference -- lags exact, magnitudes to 1e-5 of the peak.  At this size the
-    reference's last stages are off the true DFT by 5e-5, so only a decomposition that follows its stage structure passes."""
-    import subprocess, sys
-    r = subprocess.run([sys.executable, "-m", "tests.sbm_one_device", "4", "full"], capture_output=True, text=True, timeout=280,
-                       cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))), env=dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32", TSDRGPU_SBM_TIMEOUT_MS="3000"))
-    assert r.returncode == 0 and "sbm ok" in r.stdout, (r.stdout[-1500:], r.stderr[-1500:])
-    print(r.stdout[-300:])
+# The sharded path (csrc/superb_mgpu.cu) with all ranks on this GPU, and configs[3]'s 4 x 2^21, are in tests/test_superb_sweep.py.
 
 
 # ------------------------------------------------------------------------------------------------ golden vectors

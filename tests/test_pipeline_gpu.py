@@ -252,15 +252,18 @@ def run_oracle_stream_flat(O, iq, fs, h, fv):
     return w, frames
 
 
-def superb_case(H, devices=None):
+def superb_case(H, devices=None, fs=400_000, fv=50.0):
     """PARAM_AUTOCORR_SUPERRESOLUTION through the streaming pipeline: superb_run's state machine (gather H hops of 10 frames, 0.5 s
     pause and a retune after each, stitch) runs inside process(); the stitched signal then flows at H x the rate through the
     frame stages.  devices: None = all hops on one GPU (the reference's 4), else one hop per listed device (superb_mgpu.cu).
-    Returns nothing; asserts."""
+    fs / fv: the front end's rate and the refresh rate; 400 kS/s at 50 Hz gives 8000 samples per frame (nd = N/2), 819 200 S/s at
+    50 Hz gives 16 384, a power of two (nd = N).  Returns nothing; asserts."""
     from tempestsdr_b200 import pipeline
+    from tests import fft_model as fm
+    from tests import superb_model as sm
     O = orc.best()
-    fs, h, fv = 400_000, 80, 50.0
-    sif = int(fs / fv)                         # 8000 samples per frame
+    h = 80
+    sif = int(fs / fv)
     to_gather, to_pause = 10 * sif, int(0.5 * fs)
     items = 16384
     nblk = 2 * (H * (to_gather + to_pause) // (items // 2) + 8)
@@ -299,14 +302,21 @@ def superb_case(H, devices=None):
     assert st.stitches >= 1 and retunes[:H - 1] == [(k - H // 2) * fs for k in range(1, H)]     # (hop - H/2) * samplerate (superbandwidth.c:241 for H = 4)
     wH, _, _ = O.geometry(H * fs, h, fv)
     assert p.geometry()[0] == wH and len(frames) >= 4 and frames[0][1] == wH
-    # The stitched signal of the first round through the oracle's stages gives the same first frames.  Tolerance, derived: the
-    # stitch is a float32 transform, its samples agree with the reference's to eps = 1e-5 of the largest magnitude P (measured
-    # 4e-6 .. 8e-6, tests/test_gpu_parity.py); the resampler's weights sum to <= 1 per pixel, so pixels inherit eps P; auto-gain
-    # maps v -> (v - lastmin) / span with lastmin and span = lastmax - lastmin each off by up to eps P, so a delivered pixel is off by
-    # at most 3 eps P / span (first frames: span is still small because lastmax/lastmin start at 0 and move 10 % per frame).
+    # The stitched signal of the first round through the oracle's stages gives the same first frames.  Tolerance, derived: a stitched
+    # sample is within e = C_OWN_MAX u log2(H N) rms of the model of the path's own dataflow (tests/test_superb_sweep.py), and that
+    # model is within max|own - reference| of the reference's model, computed here on these hops; |.| moves nothing by more than its
+    # argument does.  The resampler's weights sum to <= 1 per pixel, so pixels inherit e; auto-gain maps v -> (v - lastmin) / span
+    # with lastmin and span = lastmax - lastmin each off by up to e, so a delivered pixel is off by at most 3 e / span (first
+    # frames: span is still small because lastmax/lastmin start at 0 and move 10 % per frame).
     want_iq, offs = O.superb_ondataready(expected_hops, sif)
     mag = O.am_demod(want_iq)
-    P = float(mag.max())
+    n_hop = fm.getrealsize(expected_hops[0].size // 2)
+    ref, _ = sm.stitch_reference(expected_hops, sif, offsets=[int(o) for o in offs])
+    if devices is None:
+        own, _ = sm.stitch_one_gpu(expected_hops, sif, offsets=[int(o) for o in offs])
+    else:
+        own, ref = sm.stitch_sharded(expected_hops, [int(o) // 2 for o in offs]), np.abs(ref)
+    e = sm.C_OWN_MAX * fm.U * fm.log2_of(H * n_hop) * fm.rms(ref) + float(np.max(np.abs(own - ref)))
     blockH = int(0.1 * H * fs / fv)
     rs = O.resampler(); pp = O.postprocessor(H * fs, h, fv, 1, 0, superres=1)
     pix = np.concatenate([rs.run(mag[k * blockH:(k + 1) * blockH], wH * h * fv, float(H * fs)) for k in range(mag.size // blockH // 10 * 10)])
@@ -315,7 +325,7 @@ def superb_case(H, devices=None):
     for k in range(min(6, pix.size // n, len(frames))):
         ref, res = pp.run(pix[k * n:(k + 1) * n], wH, h, 0.0, 0.1, 1, 0)
         got = frames[k][0]
-        tol = 3 * 1e-5 * P / (res.lastmax - res.lastmin)
+        tol = 3 * e / (res.lastmax - res.lastmin)
         err = float(np.max(np.abs(got - ref)))
         worst = max(worst, err / tol)
         assert err <= tol, f"frame {k}: {err} > {tol}"
@@ -327,17 +337,36 @@ def test_pipeline_superbandwidth_mode():
     superb_case(4, None)
 
 
+def test_pipeline_superbandwidth_mode_frames_of_a_power_of_two():
+    """819 200 S/s at 50 Hz: 16 384 samples per frame divide 2N, so the alignment correlates N points (nd = N)."""
+    superb_case(4, None, fs=819_200)
+
+
+def _superb_sharded_case(H, fs):
+    """superb_case with the hops sharded, in a process of its own: every rank's stream needs a hardware queue of its own when
+    the ranks share a GPU."""
+    import os, subprocess, sys
+    ngpu = torch.cuda.device_count()
+    devs = list(range(H)) if ngpu >= H else [0] * H
+    r = subprocess.run([sys.executable, "-c", f"from tests.test_pipeline_gpu import superb_case; superb_case({H}, {devs}, fs={fs}); print('case ok')"],
+                       capture_output=True, text=True, timeout=150, cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
+                       env=dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32", TSDRGPU_SBM_TIMEOUT_MS="1500"))
+    return r
+
+
 @pytest.mark.parametrize("H", [2, 4])
 def test_pipeline_superbandwidth_one_hop_per_device(H):
     """The same run with the hops sharded, one per device (tsdrgpu_pipeline_set_superb_devices -> superb_mgpu.cu).  On a box with
     >= H GPUs the devices are distinct (NVLink peer access); on a one-GPU box all ranks share device 0 -- same code, same flags,
-    windows in one memory.  A process of its own: every rank's stream needs a hardware queue of its own when they share a GPU."""
-    import os, subprocess, sys
-    ngpu = torch.cuda.device_count()
-    devs = list(range(H)) if ngpu >= H else [0] * H
-    r = subprocess.run([sys.executable, "-c", f"from tests.test_pipeline_gpu import superb_case; superb_case({H}, {devs}); print('case ok')"],
-                       capture_output=True, text=True, timeout=150, cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                       env=dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32", TSDRGPU_SBM_TIMEOUT_MS="1500"))
+    windows in one memory."""
+    r = _superb_sharded_case(H, 400_000)
+    assert r.returncode == 0 and "case ok" in r.stdout, (r.stdout[-1500:], r.stderr[-2500:])
+
+
+@pytest.mark.parametrize("H", [2, 4])
+def test_pipeline_superbandwidth_one_hop_per_device_frames_of_a_power_of_two(H):
+    """The sharded run at 819 200 S/s and 50 Hz: 16 384 samples per frame divide 2N, so the alignment correlates N points."""
+    r = _superb_sharded_case(H, 819_200)
     assert r.returncode == 0 and "case ok" in r.stdout, (r.stdout[-1500:], r.stderr[-2500:])
 
 
