@@ -249,6 +249,66 @@ TSDRGPU_API int  tsdrgpu_spectrum_plan(const tsdrgpu_spectrum_t *s, uint64_t pai
 TSDRGPU_API int  tsdrgpu_spectrum_run(tsdrgpu_spectrum_t *s, void *stream, const float *d_iq, uint64_t pairs, int discontinuity,
                                       double *d_reports, uint32_t capacity, uint32_t *h_nreports);
 
+/* ---------------------------------------------------------------------------- a19+  spectral coherence at the line rate (beyond the reference)
+ * An opt-in companion of the Welch spectrum that shows which of the power around a harmonic of the pixel clock is the picture.
+ * Every line of the raster carries the same horizontal blanking, so the emanation is cyclostationary at the line rate alpha: each
+ * frequency it occupies is correlated with the frequency alpha away from it.  Broadcast carriers, tones, switching spurs and receiver
+ * noise have no such correlation.  The coherence reads about 0 for them (an estimator floor of about 1/sqrt(K)) and rises where the
+ * picture's energy is.  Its axis is the spectrum's (plot 100), so the two overlay: pass the bands where it rises, stop the others.
+ * How far it rises on real captures (sync pulses, TMDS control periods) has not been measured; on synthetic video with a weak
+ * blanking level it is about 2.2 x the floor at K = 390 and 5 x at K = 3906 (DESIGN 5.5).
+ *
+ * Spec (tsdrgpu_coherence_t).  rate == 0: off.  Otherwise rate (reports per second of stream time) is an integer in
+ *   [1, TSDRGPU_COHERENCE_MAX_RATE].
+ * Cycle frequency.  alpha > 0 is the line rate in Hz: an argument of tsdrgpu_coherence_set; the pipeline uses height x refresh rate,
+ *   read at the first segment of each report (PLL steps take effect from the next report).
+ * N.  The smallest power of two with N >= 16 fs / alpha, and at least 256 (tsdrgpu_coherence_n): alpha lies 16 to 32 bins apart,
+ *   clear of the window's +-4-bin main lobe, so U+ and U- below do not overlap.  Above 65536 the spec is unresolvable: set returns
+ *   TSDRGPU_EINVAL (the pipeline delivers no coherence reports until the geometry or the sample rate changes).
+ * Window and segments: the Welch spectrum's (Blackman-Harris w of N points, hop N/2).  Segment j starts at pair s_j = j N/2, counted
+ *   from the first pair of the report in progress.
+ * Transforms and sums, for segment j:
+ *   U+-_j[k] = sum_n w+-[n] x[s_j + n] e^{-2 pi i k n/N},  w+[n] = w[n] e^{-i pi alpha n/fs},  w-[n] = conj(w+[n])
+ *   C[k] = sum_j U+_j[k] conj(U-_j[k]) e^{-2 pi i alpha s_j/fs}   (the factor makes the average coherent across segments)
+ *   P+-[k] = sum_j |U+-_j[k]|^2
+ * Report.  Each report sums K = max(1, floor(fs / (rate N/2))) segments (the tsdrgpu_spectrum_k rule), then
+ *   gamma[k] = |C[k]| / sqrt(P+[k] P-[k]) in double, 0 where P+ P- = 0.  Value i of a report is bin k = i - N/2 (fftshift order), at
+ *   (i - N/2) fs/N Hz from the tuned centre: the axis of plot 100.
+ * Discontinuities.  Unlike the Welch spectrum, a discontinuity (discontinuity != 0, the pipeline's samples_dropped != 0) discards the
+ *   open segment AND the report in progress: a gap breaks the time reference of the phase factor.  A reset, or a set with a new rate,
+ *   fs or N, also discards the report in progress; a set that changes only alpha takes effect at the next report.
+ * Computation: w+ is built in double (tsdrgpu_coherence_window) and each component rounded once to float32; x w+- is a float32
+ *   complex product with no contraction; float32 FFT with the exact DFT's stage angles; alpha s_j/fs is formed in double from the
+ *   integer s_j and reduced mod 1 before its sincospi; products, sums and gamma in double.  The same calls with the same blocks give
+ *   the same bits (no atomics). */
+#define TSDRGPU_COHERENCE_DEFAULT_RATE 1
+#define TSDRGPU_COHERENCE_MAX_RATE     100
+typedef struct {
+	int32_t rate;                                    /* reports per second of stream time; 0 = off */
+} tsdrgpu_coherence_t;
+/* host-only: the spelling shared by the host library's TSDR_COHERENCE and Python.  "off" or "line[:<rate>]" (rate default
+ * TSDRGPU_COHERENCE_DEFAULT_RATE, decimal digits only as in tsdrgpu_spectrum_parse).  TSDRGPU_OK with *out set (rate 0 for "off"),
+ * else TSDRGPU_EINVAL and *out untouched. */
+TSDRGPU_API int  tsdrgpu_coherence_parse(const char *spec, tsdrgpu_coherence_t *out);
+/* host-only: N at sample rate fs and line rate alpha (Hz); 0 when unresolvable (N > 65536) or fs == 0 or alpha is not > 0 */
+TSDRGPU_API uint32_t tsdrgpu_coherence_n(uint32_t fs, double alpha);
+/* host-only: w+ of a valid N (a power of two in [256, 65536]) in double before its rounding: 2 N values, (re, im) of each n */
+TSDRGPU_API int  tsdrgpu_coherence_window(int n, double alpha, uint32_t fs, double *w2);
+typedef struct tsdrgpu_coherence tsdrgpu_coherence_obj_t;
+TSDRGPU_API int  tsdrgpu_coherence_create(tsdrgpu_ctx_t *ctx, tsdrgpu_coherence_obj_t **c);
+TSDRGPU_API void tsdrgpu_coherence_destroy(tsdrgpu_coherence_obj_t *c);
+/* a valid spec (rate != 0), fs > 0 and alpha with tsdrgpu_coherence_n(fs, alpha) != 0, used from the next run on (alpha alone: from
+ * the next report on); a new rate, fs or N discards the open segment and the report in progress */
+TSDRGPU_API int  tsdrgpu_coherence_set(tsdrgpu_coherence_obj_t *c, const tsdrgpu_coherence_t *spec, uint32_t fs, double alpha);
+/* discards the open segment and the report in progress */
+TSDRGPU_API int  tsdrgpu_coherence_reset(tsdrgpu_coherence_obj_t *c);
+/* host-only: the number of reports the next run of `pairs` pairs would complete (state untouched) */
+TSDRGPU_API int  tsdrgpu_coherence_plan(const tsdrgpu_coherence_obj_t *c, uint64_t pairs, int discontinuity, uint32_t *nreports);
+/* asynchronous, with the contract of tsdrgpu_spectrum_run: d_iq 8-byte aligned, N doubles per report into d_reports, *h_nreports
+ * from pair counts alone, more than `capacity` reports: TSDRGPU_ECAPACITY with the state untouched.  Needs a set first. */
+TSDRGPU_API int  tsdrgpu_coherence_run(tsdrgpu_coherence_obj_t *c, void *stream, const float *d_iq, uint64_t pairs, int discontinuity,
+                                       double *d_reports, uint32_t capacity, uint32_t *h_nreports);
+
 /* ---------------------------------------------------------------------------- a6+  windowed-sinc resampler (beyond the reference)
  * An opt-in third kernel beside box (the default, above) and nearest-neighbour.  The reference chose the box integrator
  * to save CPU time; this mode evaluates the band-limited signal at the pixel instants instead.
@@ -755,6 +815,7 @@ typedef struct {
 	uint64_t h2d_bytes, d2h_bytes, gpu_launches, stitches;
 	uint64_t host_buffers_registered;   /* plugin buffers page-locked in place (cudaHostRegister) after they kept coming back */
 	uint64_t spectra_delivered, spectra_skipped;   /* spectrum reports handed to plot_cb / skipped because every report slot was busy */
+	uint64_t coherence_delivered, coherence_skipped;   /* the same for coherence reports */
 } tsdrgpu_pipeline_stats_t;
 
 typedef void (*tsdrgpu_frame_cb)(float *buf, int width, int height, void *user);                  /* tsdr_readasync_function */
@@ -843,6 +904,15 @@ TSDRGPU_API int  tsdrgpu_pipeline_set_channel(tsdrgpu_pipeline_t *p, const tsdrg
  * recorded at different tunings) discard the report in progress. */
 #define TSDRGPU_PLOT_ID_SPECTRUM 100
 TSDRGPU_API int  tsdrgpu_pipeline_set_spectrum(tsdrgpu_pipeline_t *p, const tsdrgpu_welch_t *spec);
+/* Spectral coherence of the IQ stream at the line rate (see tsdrgpu_coherence_*; NULL or rate == 0: off, the default), taking effect
+ * at the next process().  It taps where the spectrum does (after the raw-format conversion, before the channel filter, whose bands it
+ * helps to place), runs on the spectrum's low-priority stream and changes nothing else.  alpha = height x refresh rate and fs = the
+ * samplerate, read per call.  Every report goes to plot_cb(TSDRGPU_PLOT_ID_COHERENCE, -N/2, gamma, N, fs) on the delivery thread, in
+ * order; when every report slot is still held by the host that delivery is skipped (stats.coherence_skipped).  A call with
+ * samples_dropped != 0, a new samplerate or N, and superbandwidth mode (suspended for the whole mode) discard the report in
+ * progress.  While the geometry is unresolvable (tsdrgpu_coherence_n == 0) no reports are made. */
+#define TSDRGPU_PLOT_ID_COHERENCE 101
+TSDRGPU_API int  tsdrgpu_pipeline_set_coherence(tsdrgpu_pipeline_t *p, const tsdrgpu_coherence_t *spec);
 TSDRGPU_API int  tsdrgpu_pipeline_sync(tsdrgpu_pipeline_t *p, int pixels);   /* tsdr_sync: syncoffset += pixels */
 TSDRGPU_API int  tsdrgpu_pipeline_get_geometry(tsdrgpu_pipeline_t *p, int *width, int *height, double *refreshrate);
 TSDRGPU_API int  tsdrgpu_pipeline_stats(tsdrgpu_pipeline_t *p, tsdrgpu_pipeline_stats_t *out);

@@ -33,7 +33,7 @@ class PipelineStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("samples_in", "samples_dropped_upstream", "samples_resampled", "frames_processed",
                                           "frames_delivered", "frames_dropped", "captures", "plots_delivered",
                                           "h2d_bytes", "d2h_bytes", "gpu_launches", "stitches", "host_buffers_registered",
-                                          "spectra_delivered", "spectra_skipped")]
+                                          "spectra_delivered", "spectra_skipped", "coherence_delivered", "coherence_skipped")]
 
 
 FRAME_CB = C.CFUNCTYPE(None, C.POINTER(C.c_float), C.c_int, C.c_int, C.c_void_p)
@@ -100,6 +100,23 @@ def spectrum_spec(spec: str) -> WelchSpec:
     if lib().tsdrgpu_spectrum_parse(spec.encode(), C.byref(out)) != 0:
         raise ValueError(f"spectrum must be 'off' or 'welch:<N>[:<rate>]' with N a power of two in [256, 65536] and rate in "
                          f"[1, 100], not {spec!r}")
+    return out
+
+
+class CoherenceSpec(C.Structure):
+    """tsdrgpu_coherence_t"""
+    _fields_ = [("rate", C.c_int32)]
+
+
+PLOT_ID_COHERENCE = 101                             # TSDRGPU_PLOT_ID_COHERENCE
+
+
+def coherence_spec(spec: str) -> CoherenceSpec:
+    """"off" or "line[:<rate>]" (the host library's TSDR_COHERENCE spelling), read by tsdrgpu_coherence_parse.  "off" gives
+    rate == 0."""
+    out = CoherenceSpec()
+    if lib().tsdrgpu_coherence_parse(spec.encode(), C.byref(out)) != 0:
+        raise ValueError(f"coherence must be 'off' or 'line[:<rate>]' with rate in [1, 100], not {spec!r}")
     return out
 
 
@@ -202,6 +219,16 @@ _SIGS = {
     "tsdrgpu_spectrum_plan": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint32)]),
     "tsdrgpu_spectrum_run": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint32,
                                        C.POINTER(C.c_uint32)]),
+    "tsdrgpu_coherence_parse": (C.c_int, [C.c_char_p, C.POINTER(CoherenceSpec)]),
+    "tsdrgpu_coherence_n": (C.c_uint32, [C.c_uint32, C.c_double]),
+    "tsdrgpu_coherence_window": (C.c_int, [C.c_int, C.c_double, C.c_uint32, C.c_void_p]),
+    "tsdrgpu_coherence_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    "tsdrgpu_coherence_destroy": (None, [C.c_void_p]),
+    "tsdrgpu_coherence_set": (C.c_int, [C.c_void_p, C.POINTER(CoherenceSpec), C.c_uint32, C.c_double]),
+    "tsdrgpu_coherence_reset": (C.c_int, [C.c_void_p]),
+    "tsdrgpu_coherence_plan": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint32)]),
+    "tsdrgpu_coherence_run": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint32,
+                                        C.POINTER(C.c_uint32)]),
     "tsdrgpu_framestage_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "tsdrgpu_framestage_destroy": (None, [C.c_void_p]),
     "tsdrgpu_framestage_reset": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -302,6 +329,7 @@ _SIGS = {
     "tsdrgpu_pipeline_set_stack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_pipeline_set_channel": (C.c_int, [C.c_void_p, C.POINTER(ChannelSpec)]),
     "tsdrgpu_pipeline_set_spectrum": (C.c_int, [C.c_void_p, C.POINTER(WelchSpec)]),
+    "tsdrgpu_pipeline_set_coherence": (C.c_int, [C.c_void_p, C.POINTER(CoherenceSpec)]),
     "tsdrgpu_detect_videomode": (C.c_int, [C.POINTER(C.c_double), C.c_int, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_int, C.c_uint32,
                                            C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "tsdrgpu_pipeline_set_output_argb": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),

@@ -222,6 +222,9 @@ class Context:
     def spectrum(self) -> "Spectrum":
         return Spectrum(self)
 
+    def coherence(self) -> "Coherence":
+        return Coherence(self)
+
     def stack(self) -> "Stack":
         return Stack(self)
 
@@ -326,6 +329,65 @@ class Spectrum:
     def segments_per_report(spec: str, samplerate: int) -> int:
         """K of `spec` at `samplerate` (0 for "off" or samplerate 0)."""
         return N.lib().tsdrgpu_spectrum_k(C.byref(N.spectrum_spec(spec)), samplerate)
+
+
+class Coherence:
+    """The spectral coherence at the line rate of tsdrgpu.h: each segment of the Welch spectrum's segmentation transformed with the
+    complex windows w+ and w-, |sum U+ conj(U-) e^{-2 pi i alpha s/fs}| / sqrt(sum |U+|^2 sum |U-|^2) per report."""
+
+    def __init__(self, ctx: Context):
+        self.ctx = ctx
+        h = C.c_void_p()
+        ctx.chk(ctx._lib.tsdrgpu_coherence_create(ctx._h, C.byref(h)))
+        self._h = h
+        self.n = 0
+
+    def __del__(self):
+        try:
+            if self._h:
+                self.ctx._lib.tsdrgpu_coherence_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def set(self, spec: str, samplerate: int, alpha: float) -> None:
+        """"line[:<rate>]" at `samplerate` and line rate `alpha` (Hz) from the next run on; alpha alone takes effect at the next
+        report, a new rate, samplerate or N starts a new report."""
+        s = N.coherence_spec(spec)
+        if s.rate == 0:
+            raise ValueError("Coherence.set needs a 'line...' spec")
+        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_set(self._h, C.byref(s), samplerate, float(alpha)))
+        self.n = Coherence.n_for(samplerate, alpha)
+
+    def reset(self) -> None:
+        """Discard the open segment and the report in progress."""
+        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_reset(self._h))
+
+    def run(self, iq: torch.Tensor, discontinuity: bool = False) -> torch.Tensor:
+        """Interleaved float32 I,Q on the device (8-byte aligned) -> the reports this run completes, (R, N) float64 on the device in
+        fftshift order (asynchronous on the current stream).  discontinuity: these pairs do not follow the last run's."""
+        _f32(iq)
+        pairs = iq.numel() // 2
+        n = C.c_uint32(0)
+        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_plan(self._h, pairs, int(discontinuity), C.byref(n)))
+        out = torch.empty((n.value, self.n), dtype=torch.float64, device=iq.device)
+        got = C.c_uint32(0)
+        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_run(self._h, self.ctx.stream, iq.data_ptr(), pairs, int(discontinuity),
+                                                         out.data_ptr() if n.value else None, n.value, C.byref(got)))
+        assert got.value == n.value
+        return out
+
+    @staticmethod
+    def n_for(samplerate: int, alpha: float) -> int:
+        """N at `samplerate` and line rate `alpha`; 0 when unresolvable."""
+        return N.lib().tsdrgpu_coherence_n(samplerate, float(alpha))
+
+    @staticmethod
+    def window(n: int, alpha: float, samplerate: int) -> np.ndarray:
+        """w+ of N points in double, before its rounding to float32, as complex128."""
+        w = np.empty(2 * n, dtype=np.float64)
+        N.check(N.lib().tsdrgpu_coherence_window(n, float(alpha), samplerate, w.ctypes.data_as(C.c_void_p)))
+        return w[0::2] + 1j * w[1::2]
 
 
 class ChannelFilter:

@@ -53,6 +53,12 @@ struct FftPass {
 	double *acc; long long acc_bs; unsigned nseg, acc_keep;
 };
 
+// The coherence (tsdrgpu_coherence_*), beside an FftPass whose layout (and so the Welch kernels' code) it leaves alone.  Its first
+// pass reads the complex window w+ from FftPass.win as float2.  fft_acc2_kernel: transforms 2j and 2j + 1 are U+ and U- of segment
+// j, which starts at pair (seg0 + j) hop of the report; row blockIdx.y of FftPass.acc holds four planes of `plane` doubles:
+// Re C, Im C, P+, P-.
+struct CohPass { double alpha, fs; unsigned long long seg0, hop; long long plane; };
+
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
 // ---- in-register small DFTs (natural order in, natural order out) -------------------------------------------------
@@ -218,12 +224,15 @@ __device__ __forceinline__ void real_split_rn(float2 zk, float2 zm, float2 w, fl
 }
 
 // The pass over transform `by` of the batch (fft_pass_kernel: by = blockIdx.y).  RSPLIT: the first pass of the inverse half-size
-// transform (FftPass.in_real = 3) -- the forward finish happens on load.  WIN: pairs of floats (in_real = 2) are multiplied by P.win
-// on load.  ACC (fft_acc_kernel): nothing is stored; |X|^2 of every output is added to the thread's sums acc[8], which the CTA's last
-// transform (`last`) adds to its row of P.acc.
-template <int LOG2L, bool TMA, bool RSPLIT, bool ACC, bool WIN>
+// transform (FftPass.in_real = 3) -- the forward finish happens on load.  WIN = 1: pairs of floats (in_real = 2) are multiplied by
+// P.win on load; WIN = 2: by the complex window w+ in P.win (by even) or its conjugate (by odd), transform `by` reading segment
+// by / 2.  ACC = 1 (fft_acc_kernel): nothing is stored; |X|^2 of every output is added to the thread's sums acc[8], which the CTA's
+// last transform (`last`) adds to its row of P.acc.  ACC = 2 (fft_acc2_kernel): by even keeps U+ in stash[8]; by odd adds
+// U+ conj(U-) e^{i theta} (ph = (cos, sin) theta), |U+|^2 and |U-|^2 to acc[32] (four per output), written like ACC = 1 into the
+// `plane`-apart planes of the row.
+template <int LOG2L, bool TMA, bool RSPLIT, int ACC, int WIN>
 __device__ __forceinline__ void fft_pass_body(const float2 *in, float2 *out, const FftPass &P, const float2 *__restrict__ stw, unsigned by,
-                                              double *acc, bool last) {
+                                              double *acc, bool last, float2 *stash = nullptr, double2 ph = double2(), long long plane = 0) {
 	extern __shared__ __align__(128) float2 s[];
 	constexpr int L = 1 << LOG2L, NST8 = LOG2L / 3, RL = LOG2L % 3;
 	constexpr int RLAST = (RL == 0) ? 8 : ((RL == 1) ? 2 : 4);
@@ -302,13 +311,22 @@ __device__ __forceinline__ void fft_pass_body(const float2 *in, float2 *out, con
 					for (int m = 0; m < 8; m++) v[m].y = -v[m].y;
 				}
 			} else if (P.in_real == 2) {                             // pairs of floats, 4-byte aligned (a capture that starts on an odd sample)
-				const float *gr = reinterpret_cast<const float *>(in) + (long long) by * P.in_bs + 2 * (in_base + off);
+				const float *gr = reinterpret_cast<const float *>(in) + (long long) (WIN == 2 ? by >> 1 : by) * P.in_bs + 2 * (in_base + off);
 				#pragma unroll
 				for (int m = 0; m < 8; m++) v[m] = make_float2(__ldg(gr + 2 * m * step), __ldg(gr + 2 * m * step + 1));
-				if (WIN) {                                           // the window of the spectrum (tsdrgpu_spectrum_*)
+				if (WIN == 1) {                                      // the window of the spectrum (tsdrgpu_spectrum_*)
 					const float *wr = P.win + in_base + off;
 					#pragma unroll
 					for (int m = 0; m < 8; m++) { const float wv = __ldg(wr + m * step); v[m] = make_float2(__fmul_rn(v[m].x, wv), __fmul_rn(v[m].y, wv)); }
+				} else if (WIN == 2) {                               // the coherence's w+ or w- = conj(w+) (tsdrgpu_coherence_*)
+					const float2 *wr = reinterpret_cast<const float2 *>(P.win) + in_base + off;
+					const bool minus = by & 1;
+					#pragma unroll
+					for (int m = 0; m < 8; m++) {
+						const float2 wc = __ldg(wr + m * step);
+						const float wy = minus ? -wc.y : wc.y;
+						v[m] = make_float2(__fsub_rn(__fmul_rn(v[m].x, wc.x), __fmul_rn(v[m].y, wy)), __fadd_rn(__fmul_rn(v[m].x, wy), __fmul_rn(v[m].y, wc.x)));
+					}
 				}
 				if (P.conj_in) {
 					#pragma unroll
@@ -420,7 +438,30 @@ __device__ __forceinline__ void fft_pass_body(const float2 *in, float2 *out, con
 				}
 			}
 		}
-		if constexpr (ACC) {                                 // |X|^2 in double, summed over the CTA's transforms in their order
+		if constexpr (ACC == 2) {                            // the coherence's sums in double, over the CTA's segments in their order
+			if (!(by & 1)) {
+				#pragma unroll
+				for (int m = 0; m < RLAST; m++) stash[it * RLAST + m] = w[m];
+				continue;
+			}
+			double *row = P.acc + (long long) blockIdx.y * P.acc_bs + out_base + c * (int) P.out_cs;
+			#pragma unroll
+			for (int m = 0; m < RLAST; m++) {
+				const double ax = stash[it * RLAST + m].x, ay = stash[it * RLAST + m].y, bx = w[m].x, bym = w[m].y;
+				const double cr = __fma_rn(ax, bx, __dmul_rn(ay, bym)), ci = __fma_rn(ay, bx, -__dmul_rn(ax, bym));   // U+ conj(U-): exact
+				double *a = acc + 4 * (it * RLAST + m);
+				a[0] = __fma_rn(cr, ph.x, __fma_rn(-ci, ph.y, a[0]));
+				a[1] = __fma_rn(cr, ph.y, __fma_rn(ci, ph.x, a[1]));
+				a[2] = __fma_rn(ax, ax, __fma_rn(ay, ay, a[2]));
+				a[3] = __fma_rn(bx, bx, __fma_rn(bym, bym, a[3]));
+				if (last) {
+					double *d = row + (i + m * PL) * ks;
+					#pragma unroll
+					for (int q = 0; q < 4; q++) d[q * plane] = (blockIdx.y < P.acc_keep) ? __dadd_rn(d[q * plane], a[q]) : a[q];
+				}
+			}
+			continue;
+		} else if constexpr (ACC == 1) {                     // |X|^2 in double, summed over the CTA's transforms in their order
 			double *row = P.acc + (long long) blockIdx.y * P.acc_bs + out_base + c * (int) P.out_cs;
 			#pragma unroll
 			for (int m = 0; m < RLAST; m++) {
@@ -446,9 +487,9 @@ __device__ __forceinline__ void fft_pass_body(const float2 *in, float2 *out, con
 	}
 }
 
-template <int LOG2L, bool TMA = false, bool RSPLIT = false, bool WIN = false>
+template <int LOG2L, bool TMA = false, bool RSPLIT = false, int WIN = 0>
 __global__ void __launch_bounds__(512, 3) fft_pass_kernel(const float2 *in, float2 *out, FftPass P, const float2 *__restrict__ stw) {
-	fft_pass_body<LOG2L, TMA, RSPLIT, false, WIN>(in, out, P, stw, blockIdx.y, nullptr, false);
+	fft_pass_body<LOG2L, TMA, RSPLIT, 0, WIN>(in, out, P, stw, blockIdx.y, nullptr, false);
 }
 
 // The spectrum's last pass: CTA row blockIdx.y transforms blockIdx.y, blockIdx.y + gridDim.y, ... < P.nseg and adds the sum of their
@@ -461,7 +502,31 @@ __global__ void __launch_bounds__(512, 2) fft_acc_kernel(const float2 *in, FftPa
 	for (int j = 0; j < 8; j++) acc[j] = 0.0;
 	for (unsigned seg = blockIdx.y; seg < P.nseg; seg += gridDim.y) {
 		if (seg != blockIdx.y) __syncthreads();          // the last stage of the previous transform has read the shared buffers
-		fft_pass_body<LOG2L, false, false, true, true>(in, nullptr, P, stw, seg, acc, seg + gridDim.y >= P.nseg);
+		fft_pass_body<LOG2L, false, false, 1, 1>(in, nullptr, P, stw, seg, acc, seg + gridDim.y >= P.nseg);
+	}
+}
+
+// The coherence's last pass: CTA row blockIdx.y takes segments j = blockIdx.y, blockIdx.y + gridDim.y, ... < P.nseg / 2, transforms
+// 2j (U+, kept in registers) and 2j + 1 (U-) of each, and adds the per-bin sums of U+ conj(U-) e^{-2 pi i alpha s_j / fs}, |U+|^2 and
+// |U-|^2 (in that order of segments) to its row of P.acc.  alpha s_j / fs is formed in double from the integer s_j and reduced mod 1
+// before the sincospi.  One CTA per SM: the 32 double sums take 64 registers.
+template <int LOG2L>
+__global__ void __launch_bounds__(512, 1) fft_acc2_kernel(const float2 *in, FftPass P, const float2 *__restrict__ stw, CohPass Q) {
+	double acc[32];
+	float2 stash[8];
+	#pragma unroll
+	for (int j = 0; j < 32; j++) acc[j] = 0.0;
+	const unsigned nseg = P.nseg / 2;
+	for (unsigned seg = blockIdx.y; seg < nseg; seg += gridDim.y) {
+		double t = __ddiv_rn(__dmul_rn(Q.alpha, (double) ((Q.seg0 + seg) * Q.hop)), Q.fs);
+		t = __dsub_rn(t, floor(t));
+		double2 ph;
+		sincospi(__dmul_rn(-2.0, t), &ph.y, &ph.x);
+		const bool last = seg + gridDim.y >= nseg;
+		if (seg != blockIdx.y) __syncthreads();
+		fft_pass_body<LOG2L, false, false, 2, 2>(in, nullptr, P, stw, 2 * seg, acc, last, stash, ph, Q.plane);
+		__syncthreads();
+		fft_pass_body<LOG2L, false, false, 2, 2>(in, nullptr, P, stw, 2 * seg + 1, acc, last, stash, ph, Q.plane);
 	}
 }
 
@@ -659,8 +724,10 @@ int pass_attrs(tsdrgpu_ctx_t *ctx) {
 #define SET_ATTR(l) CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
 	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
 	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
-	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
-	CU_TRY(ctx, cudaFuncSetAttribute(fft_acc_kernel<l>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem))
+	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
+	CU_TRY(ctx, cudaFuncSetAttribute(fft_pass_kernel<l, false, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
+	CU_TRY(ctx, cudaFuncSetAttribute(fft_acc_kernel<l>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem)); \
+	CU_TRY(ctx, cudaFuncSetAttribute(fft_acc2_kernel<l>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem))
 	SET_ATTR(3); SET_ATTR(4); SET_ATTR(5); SET_ATTR(6); SET_ATTR(7); SET_ATTR(8); SET_ATTR(9); SET_ATTR(10); SET_ATTR(11);
 #undef SET_ATTR
 	ctx->fft_attrs_set = true;
@@ -731,8 +798,9 @@ int bundle_for(int log2L, unsigned long long lines, bool contiguous_lines = fals
 	return C < 1 ? 1 : C;
 }
 
+// coh: the coherence's passes (P.win is w+; P.acc: fft_acc2_kernel)
 int launch_pass(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, FftPass P, unsigned bundles, int inverse,
-                unsigned batch, long long in_bs, long long out_bs, const double *eps_all = NULL, int l_base = 0) {
+                unsigned batch, long long in_bs, long long out_bs, const double *eps_all = NULL, int l_base = 0, const CohPass *coh = NULL) {
 	P.in_bs = in_bs; P.out_bs = out_bs;
 	P.log2C = 0; while ((1 << P.log2C) < P.C) P.log2C++;
 	const int L = 1 << P.log2L, total = P.C * L;
@@ -764,8 +832,10 @@ int launch_pass(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float
 	                 && ((reinterpret_cast<unsigned long long>(in) | ((unsigned long long) in_bs * 8ull)) & 15ull) == 0;
 	const size_t smem = sizeof(float2) * (size_t) total * ((nstages >= 3 || (tma && nstages == 2)) ? 2 : 1);
 	switch (P.log2L) {
-#define CASE(l) case l: if (P.acc) KL(ctx, "fft_acc_kernel", stream, fft_acc_kernel<l><<<grid, threads, smem, stream>>>(in, P, stw)); \
-	                else if (P.win) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, false, true><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
+#define CASE(l) case l: if (coh && P.acc) KL(ctx, "fft_acc2_kernel", stream, fft_acc2_kernel<l><<<grid, threads, smem, stream>>>(in, P, stw, *coh)); \
+	                else if (coh) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, false, 2><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
+	                else if (P.acc) KL(ctx, "fft_acc_kernel", stream, fft_acc_kernel<l><<<grid, threads, smem, stream>>>(in, P, stw)); \
+	                else if (P.win) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, false, 1><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
 	                else if (P.in_real == 3) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false, true><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
 	                else if (tma) KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, true><<<grid, threads, smem, stream>>>(in, out, P, stw)); \
 	                else KL(ctx, "fft_pass_kernel", stream, fft_pass_kernel<l, false><<<grid, threads, smem, stream>>>(in, out, P, stw)); break
@@ -789,6 +859,9 @@ struct FftOpts {
 	// one- and two-pass plans: the last pass sums |X|^2 of the `batch` transforms into acc_rows rows of acc instead of writing `data`
 	// (fft_acc_kernel; acc_rows <= batch)
 	double *acc; long long acc_bs; unsigned acc_rows, acc_keep;
+	// the coherence: pair_in only, the complex window cwin (FftPass.win, batch = 2 x segments); with acc, the last pass is
+	// fft_acc2_kernel
+	const float2 *cwin; CohPass coh;
 };
 
 // N-point transform of `data` (complex, natural order) through `scratch`; result lands in `data`.
@@ -803,7 +876,8 @@ int fft_run(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, float2 *scrat
 	const double *eps_all = o.exact ? NULL : eps_ref;
 	FftPass P; memset(&P, 0, sizeof P);
 	P.rs_last = o.split_last; P.rs_half = (unsigned) N; P.rs_scale = o.split_scale;     // (read by the first pass only, with in_real = 3)
-	P.win = o.win;
+	P.win = o.cwin ? reinterpret_cast<const float *>(o.cwin) : o.win;
+	const CohPass *coh = o.cwin ? &o.coh : NULL;
 	// the last pass of an accumulating plan: grid.y = acc_rows CTA rows walk the `batch` transforms
 	auto accumulate = [&](FftPass &Z) { Z.acc = o.acc; Z.acc_bs = o.acc_bs; Z.nseg = o.batch; Z.acc_keep = o.acc_keep; return o.acc ? o.acc_rows : o.batch; };
 	if (log2N <= FFT_MAX_LOG2L) {                       // one pass, one CTA
@@ -811,7 +885,7 @@ int fft_run(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, float2 *scrat
 		P.in_real = in_mode; P.out_abs = o.out_abs;
 		P.conj_in = P.conj_out = inverse ? 1 : 0;
 		const unsigned rows = accumulate(P);
-		return launch_pass(ctx, stream, src0, data, P, 1, inverse, rows, in0_bs, o.data_bs, eps_all, 0);
+		return launch_pass(ctx, stream, src0, data, P, 1, inverse, rows, in0_bs, o.data_bs, eps_all, 0, coh);
 	}
 	int rc;
 	// two passes up to 2^21 (1024 x 2048: the 2048-point lines go to the contiguous pass, one TMA bulk copy per 2-line bundle);
@@ -829,7 +903,7 @@ int fft_run(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, float2 *scrat
 		P.out_lo = P.C; P.out_cs = 1; P.out_ks = (long long) N2;
 		P.tw_M = N; P.tw_lo = P.C; P.tw_cs = 1; P.scale = 1.0f; P.in_real = in_mode;
 		P.conj_in = inverse ? 1 : 0;
-		if ((rc = launch_pass(ctx, stream, src0, scratch, P, P.G_lo, inverse, o.batch, in0_bs, o.scratch_bs, eps_all, 0))) return rc;
+		if ((rc = launch_pass(ctx, stream, src0, scratch, P, P.G_lo, inverse, o.batch, in0_bs, o.scratch_bs, eps_all, 0, coh))) return rc;
 		FftPass Q; memset(&Q, 0, sizeof Q);
 		Q.log2L = (int) l2; Q.C = bundle_for((int) l2, N1, true); Q.c_fast_in = 0; Q.c_fast_out = 1;
 		Q.G_lo = (unsigned) (N1 / Q.C);
@@ -838,7 +912,7 @@ int fft_run(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, float2 *scrat
 		Q.scale = o.scale; Q.out_abs = o.out_abs;
 		Q.conj_out = inverse ? 1 : 0;
 		const unsigned rows = accumulate(Q);
-		return launch_pass(ctx, stream, scratch, data, Q, Q.G_lo, inverse, rows, o.scratch_bs, o.data_bs, eps_all, (int) l1);
+		return launch_pass(ctx, stream, scratch, data, Q, Q.G_lo, inverse, rows, o.scratch_bs, o.data_bs, eps_all, (int) l1, o.acc ? coh : NULL);
 	}
 	// N = N1*N2*N3 ; n = N2N3 n1 + N3 n2 + n3 ; k = k1 + N1 k2 + N1N2 k3
 	const unsigned l1 = (log2N + 2) / 3, l2 = (log2N - l1 + 1) / 2, l3 = log2N - l1 - l2;
@@ -1506,11 +1580,12 @@ AccShape acc_shape(unsigned log2N) {
 	a.smem = sizeof(float2) * (size_t) total * (nstages >= 3 ? 2 : 1);
 	return a;
 }
-int acc_ctas_per_sm(int log2L, int threads, size_t smem) {
+int acc_ctas_per_sm(int log2L, int threads, size_t smem, bool pair) {
 	int nb = 0;
 	cudaError_t e = cudaErrorInvalidValue;
 	switch (log2L) {
-#define CASE(l) case l: e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fft_acc_kernel<l>, threads, smem); break
+#define CASE(l) case l: e = pair ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fft_acc2_kernel<l>, threads, smem) \
+	                         : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fft_acc_kernel<l>, threads, smem); break
 	CASE(6); CASE(7); CASE(8); CASE(9); CASE(10); CASE(11);
 #undef CASE
 	default: break;
@@ -1520,19 +1595,81 @@ int acc_ctas_per_sm(int log2L, int threads, size_t smem) {
 
 }  // namespace
 
+// The segmentation the Welch spectrum and the coherence share: segments of N pairs with hop N/2, the open segment (fewer than N
+// pairs) carried across runs in d_hist, and reports of K segments.  seg_run hands the completed segments of a run to `launch` in
+// pieces of at most seg_chunk segments (all of them: 0) that stay inside one report, over at most rows_max rows of partial sums, and
+// calls `finish` for every report completed.
+struct SegStream {
+	uint32_t N, K;                                // N == 0: no spec set yet
+	DeviceBuf<float> d_hist, d_join;              // the open segment; the open segment followed by the head of a block
+	uint64_t open;                                // pairs of the open segment (in d_hist, fewer than N)
+	uint64_t done;                                // completed segments of the report in progress (< K)
+	unsigned rows_used, rows_max, seg_chunk;      // rows of partial sums that hold sums of the report in progress
+	void reset() { open = 0; done = 0; rows_used = 0; }
+	// reports the next run would complete; break_report: a discontinuity also discards the report in progress
+	uint32_t plan(uint64_t pairs, int discontinuity, bool break_report) const {
+		const uint64_t total = (discontinuity ? 0 : open) + pairs, count = total >= N ? (total - N) / (N / 2) + 1 : 0;
+		return (uint32_t) (((discontinuity && break_report ? 0 : done) + count) / K);
+	}
+	// the history buffers of N, once the work that used the old ones on `stream` is done (the caller has synchronised it)
+	cudaError_t build() { cudaError_t e = d_hist.assign(2 * (size_t) N); return e == cudaSuccess ? d_join.assign(4 * (size_t) N) : e; }
+};
+
+// launch(src, first, n, rows, keep): n consecutive segments from src (pairs, N/2 apart), segments first .. first + n - 1 of the
+// report in progress, summed into `rows` rows of which the first `keep` add to what they hold.  finish(r): report r of the run.
+template <class Launch, class Finish>
+int seg_run(tsdrgpu_ctx_t *ctx, SegStream &g, cudaStream_t stream, const float *d_iq, uint64_t pairs, int discontinuity, Launch launch,
+            Finish finish, uint32_t *h_nreports) {
+	int rc;
+	*h_nreports = 0;
+	if (discontinuity) g.open = 0;
+	if (pairs == 0) return TSDRGPU_OK;
+	const uint64_t N = g.N, H = N / 2, L = g.open, total = L + pairs;
+	const uint64_t count = total >= N ? (total - N) / H + 1 : 0;        // segments completed by this run, q = 0 .. count-1
+	const uint64_t nj = count < (L + H - 1) / H ? count : (L + H - 1) / H;   // the ones that start in the open segment
+	const uint64_t keep = total - count * H;                           // the next open segment: [count H, total)
+	// segment q starts at q H of (open segment ++ block): the first nj are formed in d_join, the others read the block in place
+	if (nj > 0 || count * H < L) {
+		const uint64_t head = pairs < N ? pairs : N;
+		if (L) CU_TRY(ctx, cudaMemcpyAsync(g.d_join.ptr, g.d_hist.ptr, sizeof(float) * 2 * L, cudaMemcpyDeviceToDevice, stream));
+		CU_TRY(ctx, cudaMemcpyAsync(g.d_join.ptr + 2 * L, d_iq, sizeof(float) * 2 * head, cudaMemcpyDeviceToDevice, stream));
+	}
+	uint32_t r = 0;
+	for (uint64_t q = 0; q < count;) {
+		const uint64_t end = q < nj ? nj : count, n = (end - q < g.K - g.done) ? end - q : g.K - g.done;
+		const float *src = q < nj ? g.d_join.ptr + 2 * q * H : d_iq + 2 * (q * H - L);
+		for (uint64_t q0 = 0; q0 < n;) {
+			const uint64_t nq = (g.seg_chunk && n - q0 > g.seg_chunk) ? g.seg_chunk : n - q0;
+			uint64_t rows = nq / SP_MIN_SEGS_PER_ROW;
+			rows = rows < 1 ? 1 : (rows > g.rows_max ? g.rows_max : rows);
+			if ((rc = launch(src + (size_t) q0 * N, g.done + q0, (unsigned) nq, (unsigned) rows, g.rows_used))) return rc;
+			if (rows > g.rows_used) g.rows_used = (unsigned) rows;
+			q0 += nq;
+		}
+		g.done += n; q += n;
+		if (g.done == g.K) {
+			if ((rc = finish(r))) return rc;
+			r++; g.done = 0; g.rows_used = 0;
+		}
+	}
+	const float *from = count * H >= L ? d_iq + 2 * (count * H - L) : g.d_join.ptr + 2 * count * H;
+	if (keep) CU_TRY(ctx, cudaMemcpyAsync(g.d_hist.ptr, from, sizeof(float) * 2 * keep, cudaMemcpyDeviceToDevice, stream));
+	g.open = keep;
+	*h_nreports = r;
+	return TSDRGPU_OK;
+}
+
 struct tsdrgpu_spectrum {
 	tsdrgpu_ctx_t *ctx;
 	tsdrgpu_welch_t spec;                         // n == 0: no spec set yet
-	uint32_t fs, K;
+	uint32_t fs;
 	double scale;                                 // 1 / (K (sum w)^2)
 	std::vector<float> h_win;                     // the float32 window of spec.n
 	int stale;                                    // the device buffers are not those of spec.n yet: the next run (re)builds them
-	DeviceBuf<float> d_win, d_hist, d_join;       // the window; the open segment; the open segment followed by the head of a block
+	SegStream seg;                                // N = spec.n, K
+	DeviceBuf<float> d_win;                       // the window
 	DeviceBuf<double> d_acc;                      // rows_max rows of N partial sums of the report in progress
 	DeviceBuf<float2> d_scratch;                  // two-pass plans: the first pass's output for seg_chunk segments
-	uint64_t open;                                // pairs of the open segment (in d_hist, fewer than N)
-	uint64_t done;                                // completed segments of the report in progress (< K)
-	unsigned rows_used, rows_max, seg_chunk;      // rows of d_acc that hold sums of the report in progress
 };
 
 extern "C" {
@@ -1554,7 +1691,7 @@ void tsdrgpu_spectrum_destroy(tsdrgpu_spectrum_t *s) {
 
 int tsdrgpu_spectrum_reset(tsdrgpu_spectrum_t *s) {
 	if (!s) return TSDRGPU_EINVAL;
-	s->open = 0; s->done = 0; s->rows_used = 0;
+	s->seg.reset();
 	return TSDRGPU_OK;
 }
 
@@ -1571,60 +1708,47 @@ int tsdrgpu_spectrum_set(tsdrgpu_spectrum_t *s, const tsdrgpu_welch_t *spec, uin
 		for (size_t i = 0; i < w.size(); i++) { s->h_win[i] = (float) w[i]; sum += (double) s->h_win[i]; }
 		s->scale = 1.0 / (sum * sum);
 		s->stale = 1;
-	} else s->scale *= (double) s->K;
+	} else s->scale *= (double) s->seg.K;
 	s->scale /= (double) K;
-	s->spec = *spec; s->fs = fs; s->K = K;
+	s->spec = *spec; s->fs = fs; s->seg.N = (uint32_t) spec->n; s->seg.K = K;
 	return tsdrgpu_spectrum_reset(s);
 }
 
 int tsdrgpu_spectrum_plan(const tsdrgpu_spectrum_t *s, uint64_t pairs, int discontinuity, uint32_t *nreports) {
 	if (!s || !nreports || s->spec.n == 0) return TSDRGPU_EINVAL;
-	const uint64_t N = (uint64_t) s->spec.n, total = (discontinuity ? 0 : s->open) + pairs;
-	const uint64_t count = total >= N ? (total - N) / (N / 2) + 1 : 0;
-	*nreports = (uint32_t) ((s->done + count) / s->K);
+	*nreports = s->seg.plan(pairs, discontinuity, false);
 	return TSDRGPU_OK;
+}
+
+}  // extern "C"
+
+// rows_max and seg_chunk of an N-point plan whose last pass is `acc_kernel_ctas` CTAs per SM and whose first pass writes
+// `per_seg` transforms per segment to the scratch
+static void seg_shape(tsdrgpu_ctx_t *ctx, SegStream &g, int ctas_per_sm, unsigned bundles, unsigned per_seg) {
+	const unsigned ctas = (unsigned) ctas_per_sm * (unsigned) ctx->sm_count;
+	const unsigned long long NP = (unsigned long long) g.N * per_seg;
+	g.rows_max = ctas / bundles > 0 ? ctas / bundles : 1;
+	g.seg_chunk = ilog2(g.N) <= (unsigned) FFT_MAX_LOG2L ? 0u : (unsigned) (SP_SCRATCH_POINTS / NP > 0 ? SP_SCRATCH_POINTS / NP : 1);
 }
 
 // the device buffers of spec.n, once the work that used the old ones on `stream` is done
 static int spectrum_build(tsdrgpu_spectrum *s, cudaStream_t stream) {
 	tsdrgpu_ctx_t *ctx = s->ctx;
 	const size_t N = (size_t) s->spec.n;
-	const unsigned log2N = ilog2(N);
-	const AccShape a = acc_shape(log2N);
+	const AccShape a = acc_shape(ilog2(N));
 	{ std::lock_guard<std::mutex> lock(ctx->mu); if (const int rc = pass_attrs(ctx)) return rc; }     // the occupancy below depends on it
-	const unsigned ctas = (unsigned) acc_ctas_per_sm(a.log2L, a.threads, a.smem) * (unsigned) ctx->sm_count;
-	s->rows_max = ctas / a.bundles > 0 ? ctas / a.bundles : 1;
-	s->seg_chunk = log2N <= (unsigned) FFT_MAX_LOG2L ? 0u : (unsigned) (SP_SCRATCH_POINTS / N > 0 ? SP_SCRATCH_POINTS / N : 1);
+	seg_shape(ctx, s->seg, acc_ctas_per_sm(a.log2L, a.threads, a.smem, false), a.bundles, 1);
 	CU_TRY(ctx, cudaStreamSynchronize(stream));
 	CU_TRY(ctx, s->d_win.assign(N));
-	CU_TRY(ctx, s->d_hist.assign(2 * N));
-	CU_TRY(ctx, s->d_join.assign(4 * N));
-	CU_TRY(ctx, s->d_acc.assign((size_t) s->rows_max * N));
-	if (s->seg_chunk) CU_TRY(ctx, s->d_scratch.assign((size_t) s->seg_chunk * N));
+	CU_TRY(ctx, s->seg.build());
+	CU_TRY(ctx, s->d_acc.assign((size_t) s->seg.rows_max * N));
+	if (s->seg.seg_chunk) CU_TRY(ctx, s->d_scratch.assign((size_t) s->seg.seg_chunk * N));
 	CU_TRY(ctx, cudaMemcpyAsync(s->d_win.ptr, s->h_win.data(), sizeof(float) * N, cudaMemcpyHostToDevice, stream));
 	s->stale = 0;
 	return TSDRGPU_OK;
 }
 
-// n consecutive segments from src (pairs, N/2 apart) into the report in progress
-static int spectrum_accumulate(tsdrgpu_spectrum *s, cudaStream_t stream, const float *src, uint64_t n) {
-	const unsigned long long N = (unsigned long long) s->spec.n;
-	for (uint64_t q0 = 0; q0 < n;) {
-		const uint64_t nq = (s->seg_chunk && n - q0 > s->seg_chunk) ? s->seg_chunk : n - q0;
-		uint64_t rows = nq / SP_MIN_SEGS_PER_ROW;
-		rows = rows < 1 ? 1 : (rows > s->rows_max ? s->rows_max : rows);
-		FftOpts o; memset(&o, 0, sizeof o);
-		o.scale = 1.0f; o.batch = (unsigned) nq; o.exact = true; o.win = s->d_win.ptr;
-		o.pair_in = src + (size_t) q0 * N; o.pair_bs = (long long) N;
-		o.scratch_bs = (long long) N;
-		o.acc = s->d_acc.ptr; o.acc_bs = (long long) N; o.acc_rows = (unsigned) rows; o.acc_keep = s->rows_used;
-		const int rc = fft_run(s->ctx, stream, NULL, s->d_scratch.ptr, ilog2(N), 0, o);
-		if (rc) return rc;
-		if (rows > s->rows_used) s->rows_used = (unsigned) rows;
-		q0 += nq;
-	}
-	return TSDRGPU_OK;
-}
+extern "C" {
 
 int tsdrgpu_spectrum_run(tsdrgpu_spectrum_t *s, void *stream_, const float *d_iq, uint64_t pairs, int discontinuity,
                          double *d_reports, uint32_t capacity, uint32_t *h_nreports) {
@@ -1641,36 +1765,166 @@ int tsdrgpu_spectrum_run(tsdrgpu_spectrum_t *s, void *stream_, const float *d_iq
 	ARG_TRY(ctx, nrep == 0 || d_reports != NULL);
 	int rc;
 	if (s->stale && (rc = spectrum_build(s, stream))) return rc;
-	*h_nreports = 0;
-	if (discontinuity) s->open = 0;
-	if (pairs == 0) return TSDRGPU_OK;
-	const uint64_t N = (uint64_t) s->spec.n, H = N / 2, L = s->open, total = L + pairs;
-	const uint64_t count = total >= N ? (total - N) / H + 1 : 0;        // segments completed by this run, q = 0 .. count-1
-	const uint64_t nj = count < (L + H - 1) / H ? count : (L + H - 1) / H;   // the ones that start in the open segment
-	const uint64_t keep = total - count * H;                           // the next open segment: [count H, total)
-	// segment q starts at q H of (open segment ++ block): the first nj are formed in d_join, the others read the block in place
-	if (nj > 0 || count * H < L) {
-		const uint64_t head = pairs < N ? pairs : N;
-		if (L) CU_TRY(ctx, cudaMemcpyAsync(s->d_join.ptr, s->d_hist.ptr, sizeof(float) * 2 * L, cudaMemcpyDeviceToDevice, stream));
-		CU_TRY(ctx, cudaMemcpyAsync(s->d_join.ptr + 2 * L, d_iq, sizeof(float) * 2 * head, cudaMemcpyDeviceToDevice, stream));
-	}
-	uint32_t r = 0;
-	for (uint64_t q = 0; q < count;) {
-		const uint64_t end = q < nj ? nj : count, n = (end - q < s->K - s->done) ? end - q : s->K - s->done;
-		const float *src = q < nj ? s->d_join.ptr + 2 * q * H : d_iq + 2 * (q * H - L);
-		if ((rc = spectrum_accumulate(s, stream, src, n))) return rc;
-		s->done += n; q += n;
-		if (s->done == s->K) {
-			KL(ctx, "k_spectrum_finish", stream, k_spectrum_finish<<<grid1d(N, ctx->sm_count), 256, 0, stream>>>(
-				s->d_acc.ptr, (long long) N, s->rows_used, (unsigned) N, s->scale, d_reports + (size_t) r * N));
-			r++; s->done = 0; s->rows_used = 0;
+	const unsigned long long N = (unsigned long long) s->spec.n;
+	auto launch = [&](const float *src, uint64_t, unsigned nq, unsigned rows, unsigned keep) -> int {
+		FftOpts o; memset(&o, 0, sizeof o);
+		o.scale = 1.0f; o.batch = nq; o.exact = true; o.win = s->d_win.ptr;
+		o.pair_in = src; o.pair_bs = (long long) N;
+		o.scratch_bs = (long long) N;
+		o.acc = s->d_acc.ptr; o.acc_bs = (long long) N; o.acc_rows = rows; o.acc_keep = keep;
+		return fft_run(ctx, stream, NULL, s->d_scratch.ptr, ilog2(N), 0, o);
+	};
+	auto finish = [&](uint32_t r) -> int {
+		KL(ctx, "k_spectrum_finish", stream, k_spectrum_finish<<<grid1d(N, ctx->sm_count), 256, 0, stream>>>(
+			s->d_acc.ptr, (long long) N, s->seg.rows_used, (unsigned) N, s->scale, d_reports + (size_t) r * N));
+		return TSDRGPU_OK;
+	};
+	return seg_run(ctx, s->seg, stream, d_iq, pairs, discontinuity, launch, finish, h_nreports);
+}
+
+}  // extern "C"
+
+// ---- spectral coherence at the line rate (definition in tsdrgpu.h) --------------------------------------------------------------
+// Each segment is transformed twice, as a batch of two (x w+ and x w-, the complex window applied on load), and fft_acc2_kernel
+// takes both transforms of a segment in one CTA, so the cross term never goes to HBM.  Rows of partial sums as in the spectrum;
+// k_coherence_finish adds them in order.
+namespace {
+
+// rows 0 .. rows-1 of acc (four planes of n each) added in order, gamma of bin (i + N/2) mod N into value i
+__global__ void __launch_bounds__(256) k_coherence_finish(const double *__restrict__ acc, long long acc_bs, unsigned rows, unsigned n,
+                                                          double *__restrict__ out) {
+	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+		const unsigned k = (i + n / 2) & (n - 1);
+		double cr = 0.0, ci = 0.0, pp = 0.0, pm = 0.0;
+		for (unsigned r = 0; r < rows; r++) {
+			const double *a = acc + (long long) r * acc_bs + k;
+			cr = __dadd_rn(cr, a[0]); ci = __dadd_rn(ci, a[n]); pp = __dadd_rn(pp, a[2 * n]); pm = __dadd_rn(pm, a[3 * n]);
 		}
+		const double den = __dmul_rn(pp, pm);
+		out[i] = den > 0.0 ? __ddiv_rn(__dsqrt_rn(__fma_rn(cr, cr, __dmul_rn(ci, ci))), __dsqrt_rn(den)) : 0.0;
 	}
-	const float *from = count * H >= L ? d_iq + 2 * (count * H - L) : s->d_join.ptr + 2 * count * H;
-	if (keep) CU_TRY(ctx, cudaMemcpyAsync(s->d_hist.ptr, from, sizeof(float) * 2 * keep, cudaMemcpyDeviceToDevice, stream));
-	s->open = keep;
-	*h_nreports = r;
+}
+
+}  // namespace
+
+struct tsdrgpu_coherence {
+	tsdrgpu_ctx_t *ctx;
+	tsdrgpu_coherence_t spec;                     // rate == 0: no spec set yet
+	uint32_t fs;
+	double alpha;                                 // the last set's; the report in progress uses alpha_rep
+	double alpha_rep;                             // the alpha whose window is in d_cwin (0: none yet)
+	int stale;                                    // the device buffers are not those of seg.N yet: the next run (re)builds them
+	SegStream seg;
+	DeviceBuf<float2> d_cwin;                     // w+ of alpha_rep
+	DeviceBuf<double> d_acc;                      // rows_max rows of 4 N partial sums (Re C, Im C, P+, P-) of the report in progress
+	DeviceBuf<float2> d_scratch;                  // two-pass plans: the first pass's output for seg_chunk segments (2 transforms each)
+	std::vector<float2> h_cwin;
+};
+
+extern "C" {
+
+int tsdrgpu_coherence_create(tsdrgpu_ctx_t *ctx, tsdrgpu_coherence_obj_t **out) {
+	BIND(ctx); ARG_TRY(ctx, out != NULL);
+	tsdrgpu_coherence *c = new tsdrgpu_coherence();    // value-initialised; buffers are sized by the first run after a set
+	c->ctx = ctx;
+	*out = c;
 	return TSDRGPU_OK;
+}
+
+void tsdrgpu_coherence_destroy(tsdrgpu_coherence_obj_t *c) {
+	if (!c) return;
+	cudaSetDevice(c->ctx->device);
+	cudaDeviceSynchronize();
+	delete c;
+}
+
+int tsdrgpu_coherence_reset(tsdrgpu_coherence_obj_t *c) {
+	if (!c) return TSDRGPU_EINVAL;
+	c->seg.reset();
+	return TSDRGPU_OK;
+}
+
+int tsdrgpu_coherence_set(tsdrgpu_coherence_obj_t *c, const tsdrgpu_coherence_t *spec, uint32_t fs, double alpha) {
+	if (!c) return TSDRGPU_EINVAL;
+	const uint32_t N = tsdrgpu_coherence_n(fs, alpha);
+	const tsdrgpu_welch_t w = {(int32_t) N, spec ? spec->rate : 0};
+	const uint32_t K = N ? tsdrgpu_spectrum_k(&w, fs) : 0;
+	if (K == 0) return tsdrgpu_fail(c->ctx, TSDRGPU_EINVAL, "invalid coherence spec, sample rate or line rate (tsdrgpu.h)", cudaSuccess, __FILE__, __LINE__);
+	c->alpha = alpha;                             // alone: from the next report on
+	if (spec->rate == c->spec.rate && fs == c->fs && N == c->seg.N) return TSDRGPU_OK;
+	if (N != c->seg.N) c->stale = 1;
+	c->alpha_rep = 0;                             // the window depends on fs: rebuilt at the next report
+	c->spec = *spec; c->fs = fs; c->seg.N = N; c->seg.K = K;
+	return tsdrgpu_coherence_reset(c);
+}
+
+int tsdrgpu_coherence_plan(const tsdrgpu_coherence_obj_t *c, uint64_t pairs, int discontinuity, uint32_t *nreports) {
+	if (!c || !nreports || c->spec.rate == 0) return TSDRGPU_EINVAL;
+	*nreports = c->seg.plan(pairs, discontinuity, true);
+	return TSDRGPU_OK;
+}
+
+}  // extern "C"
+
+static int coherence_build(tsdrgpu_coherence *c, cudaStream_t stream) {
+	tsdrgpu_ctx_t *ctx = c->ctx;
+	const size_t N = c->seg.N;
+	const AccShape a = acc_shape(ilog2(N));
+	{ std::lock_guard<std::mutex> lock(ctx->mu); if (const int rc = pass_attrs(ctx)) return rc; }
+	seg_shape(ctx, c->seg, acc_ctas_per_sm(a.log2L, a.threads, a.smem, true), a.bundles, 2);
+	CU_TRY(ctx, cudaStreamSynchronize(stream));
+	CU_TRY(ctx, c->d_cwin.assign(N));
+	CU_TRY(ctx, c->seg.build());
+	CU_TRY(ctx, c->d_acc.assign((size_t) c->seg.rows_max * 4 * N));
+	if (c->seg.seg_chunk) CU_TRY(ctx, c->d_scratch.assign((size_t) c->seg.seg_chunk * 2 * N));
+	c->alpha_rep = 0;
+	c->stale = 0;
+	return TSDRGPU_OK;
+}
+
+extern "C" {
+
+int tsdrgpu_coherence_run(tsdrgpu_coherence_obj_t *c, void *stream_, const float *d_iq, uint64_t pairs, int discontinuity,
+                          double *d_reports, uint32_t capacity, uint32_t *h_nreports) {
+	ARG_TRY((tsdrgpu_ctx_t *) NULL, c != NULL);
+	tsdrgpu_ctx_t *ctx = c->ctx;
+	BIND(ctx);
+	cudaStream_t stream = (cudaStream_t) stream_;
+	if (c->spec.rate == 0) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "coherence run before a spec was set", cudaSuccess, __FILE__, __LINE__);
+	ARG_TRY(ctx, h_nreports != NULL && pairs <= (1ull << 40));
+	ARG_TRY(ctx, pairs == 0 || (d_iq != NULL && ((uintptr_t) d_iq & 7u) == 0));
+	uint32_t nrep = 0;
+	tsdrgpu_coherence_plan(c, pairs, discontinuity, &nrep);
+	if (nrep > capacity) return tsdrgpu_fail(ctx, TSDRGPU_ECAPACITY, "coherence run: more reports than the output holds", cudaSuccess, __FILE__, __LINE__);
+	ARG_TRY(ctx, nrep == 0 || d_reports != NULL);
+	int rc;
+	if (c->stale && (rc = coherence_build(c, stream))) return rc;
+	if (discontinuity) { c->seg.done = 0; c->seg.rows_used = 0; }      // the time reference of the report is lost with the run
+	const unsigned long long N = c->seg.N;
+	auto launch = [&](const float *src, uint64_t first, unsigned nq, unsigned rows, unsigned keep) -> int {
+		if (first == 0 && c->alpha_rep != c->alpha) {                   // alpha is read at the first segment of a report
+			std::vector<double> w2(2 * N);
+			tsdrgpu_coherence_window((int) N, c->alpha, c->fs, w2.data());
+			c->h_cwin.resize(N);
+			for (size_t i = 0; i < N; i++) c->h_cwin[i] = make_float2((float) w2[2 * i], (float) w2[2 * i + 1]);
+			// pageable source: the copy has taken the host values when it returns
+			CU_TRY(ctx, cudaMemcpyAsync(c->d_cwin.ptr, c->h_cwin.data(), sizeof(float2) * N, cudaMemcpyHostToDevice, stream));
+			c->alpha_rep = c->alpha;
+		}
+		FftOpts o; memset(&o, 0, sizeof o);
+		o.scale = 1.0f; o.batch = 2 * nq; o.exact = true; o.cwin = c->d_cwin.ptr;
+		o.pair_in = src; o.pair_bs = (long long) N;
+		o.scratch_bs = (long long) N;
+		o.acc = c->d_acc.ptr; o.acc_bs = 4 * (long long) N; o.acc_rows = rows; o.acc_keep = keep;
+		o.coh.alpha = c->alpha_rep; o.coh.fs = (double) c->fs; o.coh.seg0 = first; o.coh.hop = N / 2; o.coh.plane = (long long) N;
+		return fft_run(ctx, stream, NULL, c->d_scratch.ptr, ilog2(N), 0, o);
+	};
+	auto finish = [&](uint32_t r) -> int {
+		KL(ctx, "k_coherence_finish", stream, k_coherence_finish<<<grid1d(N, ctx->sm_count), 256, 0, stream>>>(
+			c->d_acc.ptr, 4 * (long long) N, c->seg.rows_used, (unsigned) N, d_reports + (size_t) r * N));
+		return TSDRGPU_OK;
+	};
+	return seg_run(ctx, c->seg, stream, d_iq, pairs, discontinuity, launch, finish, h_nreports);
 }
 
 }  // extern "C"

@@ -196,6 +196,42 @@ uint32_t tsdrgpu_spectrum_k(const tsdrgpu_welch_t *spec, uint32_t fs) {
 	return k > 0 ? (uint32_t) k : 1u;
 }
 
+/* ---- the coherence's spelling, N and window (definitions in tsdrgpu.h) */
+int tsdrgpu_coherence_parse(const char *spec, tsdrgpu_coherence_t *out) {
+	if (!spec || !out) return TSDRGPU_EINVAL;
+	tsdrgpu_coherence_t s = {0};
+	if (strcmp(spec, "off") == 0) { *out = s; return TSDRGPU_OK; }
+	const char *c = spec;
+	if (strncmp(c, "line", 4) != 0) return TSDRGPU_EINVAL;
+	c += 4;
+	s.rate = TSDRGPU_COHERENCE_DEFAULT_RATE;
+	if (*c == ':') { c++; if (!spectrum_digits(&c, &s.rate)) return TSDRGPU_EINVAL; }
+	if (*c || s.rate < 1 || s.rate > TSDRGPU_COHERENCE_MAX_RATE) return TSDRGPU_EINVAL;
+	*out = s;
+	return TSDRGPU_OK;
+}
+
+uint32_t tsdrgpu_coherence_n(uint32_t fs, double alpha) {
+	if (fs == 0 || !(alpha > 0.0) || alpha > 1e300) return 0;
+	const double need = 16.0 * (double) fs / alpha;
+	uint32_t n = TSDRGPU_SPECTRUM_MIN_N;
+	while ((double) n < need) { if (n >= TSDRGPU_SPECTRUM_MAX_N) return 0; n *= 2; }
+	return n;
+}
+
+int tsdrgpu_coherence_window(int n, double alpha, uint32_t fs, double *w2) {
+	const tsdrgpu_welch_t s = {n, 1};
+	if (!w2 || !spectrum_valid(&s) || fs == 0 || !(alpha > 0.0) || alpha > 1e300) return TSDRGPU_EINVAL;
+	const double pi = 3.14159265358979323846;
+	tsdrgpu_spectrum_window(n, w2 + n);                /* the real window in the upper half, read before it is overwritten */
+	for (int i = 0; i < n; i++) {
+		const double w = w2[n + i], a = -pi * fmod(alpha * (double) i / (double) fs, 2.0);
+		w2[2 * i] = w * cos(a);
+		w2[2 * i + 1] = w * sin(a);
+	}
+	return TSDRGPU_OK;
+}
+
 /* ---- auto-gain, contrast, denoise, stack and deblur options (definitions in tsdrgpu.h) */
 int autogain_ok(int mode, int ppm) {
 	return (mode == TSDRGPU_AG_MINMAX || mode == TSDRGPU_AG_CLIP) && ppm >= 0 && ppm <= TSDRGPU_AG_MAX_PPM;

@@ -34,9 +34,9 @@ namespace {
 constexpr int PL_SLOTS = 4;
 
 struct FrameJob {
-	int kind;                 // 0 = frames, 1 = plots, 2 = barrier, 3 = a spectrum report
+	int kind;                 // 0 = frames, 1 = plots, 2 = barrier, 3 = a spectrum report, 4 = a coherence report
 	int slot, nframes, w, h;
-	int spec_n;               // spectrum report: N
+	int spec_n;               // spectrum or coherence report: N
 	cudaEvent_t ev;
 	uint32_t samplerate;      // plots
 	int foff, flen, loff, llen; uint64_t calls; int reset_announce, dump_announce;
@@ -67,6 +67,7 @@ struct Settings {
 	int stack_restart = 0;                             // tsdr_sync: the stack restarts at the next frame-stage batch
 	tsdrgpu_channel_t cf_spec = {};                    // taps == 0: off; applied per process()
 	tsdrgpu_welch_t sp_spec = {};                      // n == 0: off; applied per process()
+	tsdrgpu_coherence_t ch_spec = {};                  // rate == 0: off; applied per process()
 	int host_register = 0;                             // opt-in: tsdrgpu_pipeline_set_host_registration
 	tsdrgpu_retune_cb retune_cb = nullptr;
 };
@@ -177,9 +178,12 @@ struct tsdrgpu_pipeline {
 	int cf_stale;                                      // a block with samples went by unfiltered: zero the history before the next
 	// Welch spectrum (tsdrgpu_pipeline_set_spectrum): the object is created on first use, its work runs on s_spec (low priority)
 	tsdrgpu_spectrum *sp; cudaStream_t s_spec;
-	cudaEvent_t ev_conv, ev_sp_used[4];                // the block is converted / the spectrum has read staging slot i
+	cudaEvent_t ev_conv, ev_sp_used[4];                // the block is converted / s_spec (spectrum, coherence) has read staging slot i
 	DeviceBuf<double> d_sp_out; PinnedBuf<double> h_spec[PL_SLOTS]; int spec_busy[PL_SLOTS];
 	int sp_fresh;                                      // blocks went by without the spectrum: the next one starts a new report
+	// coherence (tsdrgpu_pipeline_set_coherence): as the spectrum, on s_spec; ev_sp_used covers both readers of a staging slot
+	tsdrgpu_coherence *ch; DeviceBuf<double> d_ch_out; PinnedBuf<double> h_coh[PL_SLOTS]; int coh_busy[PL_SLOTS];
+	int ch_fresh;
 	DeviceBuf<float> d_pix; size_t pix_read, pix_fill;
 	DropComp pix_drop;
 	// stage 3: frames
@@ -287,6 +291,11 @@ static void *delivery_main(void *arg) {
 			if (p->plot_cb) p->plot_cb(TSDRGPU_PLOT_ID_SPECTRUM, -j.spec_n / 2, p->h_spec[j.slot].ptr, j.spec_n, j.samplerate, p->user);
 			pthread_mutex_lock(&p->mu);
 			p->spec_busy[j.slot] = 0; p->stats.spectra_delivered++;
+			pthread_mutex_unlock(&p->mu);
+		} else if (j.kind == 4) {
+			if (p->plot_cb) p->plot_cb(TSDRGPU_PLOT_ID_COHERENCE, -j.spec_n / 2, p->h_coh[j.slot].ptr, j.spec_n, j.samplerate, p->user);
+			pthread_mutex_lock(&p->mu);
+			p->coh_busy[j.slot] = 0; p->stats.coherence_delivered++;
 			pthread_mutex_unlock(&p->mu);
 		}
 		cudaEventDestroy(j.ev);
@@ -664,7 +673,7 @@ static int create_handles(tsdrgpu_pipeline *p) {
 // thread must not be running and the pipeline's device must be current.
 static void release(tsdrgpu_pipeline *p) {
 	tsdrgpu_resampler_destroy(p->rs); tsdrgpu_framestage_destroy(p->fs); tsdrgpu_frd_destroy(p->frd); tsdrgpu_chanfilt_destroy(p->cf);
-	tsdrgpu_spectrum_destroy(p->sp);
+	tsdrgpu_spectrum_destroy(p->sp); tsdrgpu_coherence_destroy(p->ch);
 	for (auto &b : p->hostbufs) if (b.state == 1) { cudaHostUnregister(const_cast<void *>(b.base)); cudaGetLastError(); }
 	superb_release(p);
 	for (cudaStream_t *s : own_streams(p)) if (*s) cudaStreamDestroy(*s);
@@ -778,6 +787,16 @@ int tsdrgpu_pipeline_set_spectrum(tsdrgpu_pipeline_t *p, const tsdrgpu_welch_t *
 		w = *spec;
 	}
 	return update(p, true, [&](Settings &s) { s.sp_spec = w; });
+}
+int tsdrgpu_pipeline_set_coherence(tsdrgpu_pipeline_t *p, const tsdrgpu_coherence_t *spec) {
+	if (!p) return TSDRGPU_EINVAL;
+	tsdrgpu_coherence_t c = {0};
+	if (spec && spec->rate != 0) {
+		if (spec->rate < 1 || spec->rate > TSDRGPU_COHERENCE_MAX_RATE)
+			return tsdrgpu_fail(p->ctx, TSDRGPU_EINVAL, "invalid coherence spec (tsdrgpu.h)", cudaSuccess, __FILE__, __LINE__);
+		c = *spec;
+	}
+	return update(p, true, [&](Settings &s) { s.ch_spec = c; });
 }
 int tsdrgpu_pipeline_set_denoise(tsdrgpu_pipeline_t *p, int mode, int h_milli, int r, int p_radius) {
 	return update(p, denoise_ok(mode, h_milli, r, p_radius), [&](Settings &s) {
@@ -987,9 +1006,9 @@ static int channel_filter(tsdrgpu_pipeline *p, const tsdrgpu_channel_t *spec, ui
 	return tsdrgpu_chanfilt_run(p->cf, p->s_ingest, stage, pairs, p->d_cf_out.ptr);
 }
 
-// the spectrum over one whole converted block (staging slot ss) on s_spec, its reports copied into free report slots and queued for
-// delivery.  ev_sp_used[ss] keeps the copy four calls later from overwriting the slot before the spectrum has read it.
-static int spectrum_block(tsdrgpu_pipeline *p, const Settings &s, const float *stage, uint64_t pairs, bool dropped, int ss) {
+// the spectrum over one whole converted block on s_spec (after ev_conv), its reports copied into free report slots and queued for
+// delivery
+static int spectrum_block(tsdrgpu_pipeline *p, const Settings &s, const float *stage, uint64_t pairs, bool dropped) {
 	tsdrgpu_ctx_t *ctx = p->ctx;
 	int rc;
 	if (!p->sp && (rc = tsdrgpu_spectrum_create(ctx, &p->sp))) return rc;
@@ -1011,9 +1030,7 @@ static int spectrum_block(tsdrgpu_pipeline *p, const Settings &s, const float *s
 		pthread_mutex_unlock(&p->mu);
 		for (int k = 0; k < PL_SLOTS; k++) if ((rc = p->h_spec[k].assign(ctx, N))) return rc;
 	}
-	CU_TRY(ctx, cudaStreamWaitEvent(p->s_spec, p->ev_conv, 0));
 	if ((rc = tsdrgpu_spectrum_run(p->sp, p->s_spec, stage, pairs, dropped, p->d_sp_out.ptr, nrep, &nrep))) return rc;
-	CU_TRY(ctx, cudaEventRecord(p->ev_sp_used[ss], p->s_spec));
 	for (uint32_t r = 0; r < nrep; r++) {
 		pthread_mutex_lock(&p->mu);
 		int slot = -1;
@@ -1025,6 +1042,49 @@ static int spectrum_block(tsdrgpu_pipeline *p, const Settings &s, const float *s
 		p->stats.d2h_bytes += sizeof(double) * N;
 		FrameJob j; memset(&j, 0, sizeof j);
 		j.kind = 3; j.slot = slot; j.spec_n = (int) N; j.samplerate = s.samplerate;
+		if ((rc = submit(p, j, p->s_spec))) return rc;
+	}
+	return TSDRGPU_OK;
+}
+
+// the coherence over one whole converted block on s_spec, as spectrum_block.  A geometry it cannot resolve makes no reports and
+// starts a new report once it can.
+static int coherence_block(tsdrgpu_pipeline *p, const Settings &s, const float *stage, uint64_t pairs, bool dropped) {
+	tsdrgpu_ctx_t *ctx = p->ctx;
+	int rc;
+	const double alpha = (double) s.height * s.refreshrate;
+	const size_t N = tsdrgpu_coherence_n(s.samplerate, alpha);
+	if (N == 0) { p->ch_fresh = 1; return TSDRGPU_OK; }
+	if (!p->ch && (rc = tsdrgpu_coherence_create(ctx, &p->ch))) return rc;
+	if ((rc = tsdrgpu_coherence_set(p->ch, &s.ch_spec, s.samplerate, alpha))) return rc;   // a new rate, fs or N: a new report
+	if (p->ch_fresh && (rc = tsdrgpu_coherence_reset(p->ch))) return rc;
+	p->ch_fresh = 0;
+	uint32_t nrep = 0;
+	if ((rc = tsdrgpu_coherence_plan(p->ch, pairs, dropped, &nrep))) return rc;
+	if (p->d_ch_out.cap < nrep * N) {
+		CU_TRY(ctx, cudaStreamSynchronize(p->s_spec));
+		CU_TRY(ctx, p->d_ch_out.reserve(p->s_spec, nrep * N));
+	}
+	bool regrow = false;
+	for (int k = 0; k < PL_SLOTS; k++) regrow |= p->h_coh[k].cap < N;
+	if (nrep && regrow) {
+		pthread_mutex_lock(&p->mu);
+		while (p->delivered < p->submitted) pthread_cond_wait(&p->cv_done, &p->mu);
+		pthread_mutex_unlock(&p->mu);
+		for (int k = 0; k < PL_SLOTS; k++) if ((rc = p->h_coh[k].assign(ctx, N))) return rc;
+	}
+	if ((rc = tsdrgpu_coherence_run(p->ch, p->s_spec, stage, pairs, dropped, p->d_ch_out.ptr, nrep, &nrep))) return rc;
+	for (uint32_t r = 0; r < nrep; r++) {
+		pthread_mutex_lock(&p->mu);
+		int slot = -1;
+		for (int k = 0; k < PL_SLOTS; k++) if (!p->coh_busy[k]) { slot = k; break; }
+		if (slot >= 0) p->coh_busy[slot] = 1; else p->stats.coherence_skipped++;
+		pthread_mutex_unlock(&p->mu);
+		if (slot < 0) continue;
+		CU_TRY(ctx, cudaMemcpyAsync(p->h_coh[slot].ptr, p->d_ch_out.ptr + r * N, sizeof(double) * N, cudaMemcpyDeviceToHost, p->s_spec));
+		p->stats.d2h_bytes += sizeof(double) * N;
+		FrameJob j; memset(&j, 0, sizeof j);
+		j.kind = 4; j.slot = slot; j.spec_n = (int) N; j.samplerate = s.samplerate;
 		if ((rc = submit(p, j, p->s_spec))) return rc;
 	}
 	return TSDRGPU_OK;
@@ -1061,8 +1121,9 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 	const int w = s.width, h = s.height; const double ptos = s.ptos;     // the geometry at the call's start plans its blocks
 	p->stats.samples_in += size2;
 	if (samples_dropped > 0) p->stats.samples_dropped_upstream += (uint64_t) samples_dropped;
-	const bool sp_on = s.sp_spec.n != 0;
+	const bool sp_on = s.sp_spec.n != 0, ch_on = s.ch_spec.rate != 0;
 	if (s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION] || !sp_on) p->sp_fresh = 1;      // hops at other tunings, or no spectrum
+	if (s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION] || !ch_on) p->ch_fresh = 1;
 	if (s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION]) {
 		if (size2 > 0) p->cf_stale = 1;                        // the hops are recorded unfiltered: the bands refer to one tuning
 		return superb_step(p, s, h_iq, fmt, items_count, samples_dropped);
@@ -1075,9 +1136,10 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 	const bool drop_all = p->dev_drop.will_drop_all((uint32_t) size2);
 	const bool plots_on = !s.params[TSDRGPU_PARAM_AUTOCORR_PLOTS_OFF];
 	int rc = TSDRGPU_OK;
-	// the block is needed by the decimator or the capture (need_main), or by the spectrum alone: it sees every pair delivered
+	// the block is needed by the decimator or the capture (need_main), or by the spectrum or the coherence alone: they see every
+	// pair delivered
 	const bool need_main = size2 > 0 && (!drop_all || (plots_on && samples_dropped != 0));
-	const bool need_data = need_main || (sp_on && size2 > 0);
+	const bool need_data = need_main || ((sp_on || ch_on) && size2 > 0);
 	const int ss = p->stage_slot;
 	float *stage = NULL;
 	bool copy_issued = false;
@@ -1099,7 +1161,7 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 			if (fmt != TSDRGPU_FMT_FLOAT && (rc = raw_reserve(p, ss, bytes))) break;
 			const void *src = host_source(p, s.host_register, h_iq, bytes);
 			e = cudaStreamWaitEvent(p->s_copy, p->ev_used[ss], 0);
-			if (e == cudaSuccess && p->sp) e = cudaStreamWaitEvent(p->s_copy, p->ev_sp_used[ss], 0);   // and the spectrum's read of it
+			if (e == cudaSuccess && (p->sp || p->ch)) e = cudaStreamWaitEvent(p->s_copy, p->ev_sp_used[ss], 0);   // and s_spec's reads of it
 			if (e == cudaSuccess) { e = cudaMemcpyAsync(fmt == TSDRGPU_FMT_FLOAT ? (void *) stage : p->d_raw[ss].ptr, src, bytes, cudaMemcpyHostToDevice, p->s_copy); copy_issued = true; }
 			if (e == cudaSuccess) e = cudaEventRecord(p->ev_h2d[ss], p->s_copy);
 			if (e == cudaSuccess) e = cudaStreamWaitEvent(p->s_ingest, p->ev_h2d[ss], 0);
@@ -1111,10 +1173,14 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 				if ((e = cudaGetLastError()) != cudaSuccess) { rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "kernel launch", e, __FILE__, __LINE__); break; }
 			}
 			p->stats.h2d_bytes += bytes;
-			if (sp_on) {                                                       // the converted block, before the channel filter
+			if (sp_on || ch_on) {                                              // the converted block, before the channel filter
 				e = cudaEventRecord(p->ev_conv, fmt == TSDRGPU_FMT_FLOAT ? p->s_copy : p->s_ingest);
+				if (e == cudaSuccess) e = cudaStreamWaitEvent(p->s_spec, p->ev_conv, 0);
 				if (e != cudaSuccess) { rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "stream ordering", e, __FILE__, __LINE__); break; }
-				if ((rc = spectrum_block(p, s, stage, size2, samples_dropped != 0, ss))) break;
+				if (sp_on && (rc = spectrum_block(p, s, stage, size2, samples_dropped != 0))) break;
+				if (ch_on && (rc = coherence_block(p, s, stage, size2, samples_dropped != 0))) break;
+				// ev_sp_used[ss] keeps the copy four calls later from overwriting the slot before s_spec has read it
+				if ((e = cudaEventRecord(p->ev_sp_used[ss], p->s_spec)) != cudaSuccess) { rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "stream ordering", e, __FILE__, __LINE__); break; }
 			}
 			if (need_main) {
 				if (cf_on) {                                                   // the capture and the decimator read the filtered block

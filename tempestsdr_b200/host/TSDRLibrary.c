@@ -398,6 +398,16 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 			goto end;
 		}
 	}
+	/* TSDR_COHERENCE=line[:<rate>]: the spectral coherence of the IQ stream at the line rate delivered to plot_cb as plot id
+	 * TSDRGPU_PLOT_ID_COHERENCE, on the axis of the spectrum (tsdrgpu.h).  Unset or "off": none */
+	tsdrgpu_coherence_t coherence = {0};
+	{
+		const char *co = getenv("TSDR_COHERENCE");
+		if (co && tsdrgpu_coherence_parse(co, &coherence) != TSDRGPU_OK) {
+			status = fail(t, "TSDR_COHERENCE must be \"off\" or \"line[:<rate>]\" with rate in [1, 100]", TSDR_INVALID_PARAMETER_VALUE);
+			goto end;
+		}
+	}
 	/* TSDR_DENOISE=nlm:<h>[:<R>:<P>]: non-local means of the delivered frames, ahead of CLAHE (tsdrgpu.h).  Unset or "off": none */
 	int nl_mode = TSDRGPU_DENOISE_OFF, nl_h = 0, nl_r = 0, nl_p = 0;
 	{
@@ -486,6 +496,7 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 			if (db_mode != TSDRGPU_DEBLUR_OFF) tsdrgpu_pipeline_set_deblur(np, db_mode, db_sigma, db_iters);
 			if (channel.taps != 0) tsdrgpu_pipeline_set_channel(np, &channel);
 			if (spectrum.n != 0) tsdrgpu_pipeline_set_spectrum(np, &spectrum);
+			if (coherence.rate != 0) tsdrgpu_pipeline_set_coherence(np, &coherence);
 		}
 		pthread_rwlock_wrlock(&t->pipe_lock);
 		t->pipe = np;                                 /* published: setters on other threads reach the run from here on */

@@ -26,7 +26,7 @@ class Pipeline:
                  on_frame: Optional[Callable] = None, on_value: Optional[Callable] = None, on_plot: Optional[Callable] = None,
                  on_retune: Optional[Callable] = None, resampler: str = "box", autogain: str = "minmax",
                  contrast: str = "off", channel: str = "off", denoise: str = "off", spectrum: str = "off",
-                 stack: str = "off", deblur: str = "off"):
+                 stack: str = "off", deblur: str = "off", coherence: str = "off"):
         self._lib = N.lib()
         ctx = C.c_void_p()
         N.check(self._lib.tsdrgpu_create(C.byref(ctx), device))
@@ -75,6 +75,8 @@ class Pipeline:
             self.set_denoise(denoise)
         if spectrum != "off":
             self.set_spectrum(spectrum)
+        if coherence != "off":
+            self.set_coherence(coherence)
         if stack != "off":
             self.set_stack(stack)
         if deblur != "off":
@@ -169,6 +171,12 @@ class Pipeline:
         """"off" (the default) or "welch:<N>[:<rate>]" (a Welch power spectrum of the IQ stream before the channel filter, tsdrgpu.h)
         from the next process() on.  Reports reach on_plot as (100, -N/2, N values in fftshift order, samplerate)."""
         N.check(self._lib.tsdrgpu_pipeline_set_spectrum(self._h, C.byref(N.spectrum_spec(spec))), self._ctx)
+
+    def set_coherence(self, spec: str) -> None:
+        """"off" (the default) or "line[:<rate>]" (the spectral coherence of the IQ stream at the line rate, before the channel
+        filter, tsdrgpu.h) from the next process() on.  Reports reach on_plot as (101, -N/2, N values of gamma in fftshift order,
+        samplerate), on the axis of the spectrum's plot 100."""
+        N.check(self._lib.tsdrgpu_pipeline_set_coherence(self._h, C.byref(N.coherence_spec(spec))), self._ctx)
 
     def set_param(self, name: str, value: int) -> None:
         N.check(self._lib.tsdrgpu_pipeline_set_param_int(self._h, PARAM_IDS[name], value), self._ctx)
