@@ -273,24 +273,51 @@ class Stack:
         return out, [N.StackRecord.from_buffer_copy(r) for r in recs]
 
 
-class Spectrum:
-    """The Welch power spectrum of tsdrgpu.h: windowed, 50 % overlapping segments of the IQ stream, K of them averaged per report,
-    with the open segment carried from run to run."""
+class _SegmentReports:
+    """What Spectrum and Coherence share: the object tsdrgpu_<_kind>_* of tsdrgpu.h, its reset and its runs."""
+    _kind = ""
 
     def __init__(self, ctx: Context):
         self.ctx = ctx
         h = C.c_void_p()
-        ctx.chk(ctx._lib.tsdrgpu_spectrum_create(ctx._h, C.byref(h)))
+        ctx.chk(self._fn("create")(ctx._h, C.byref(h)))
         self._h = h
         self.n = 0
+
+    def _fn(self, name: str):
+        return getattr(self.ctx._lib, f"tsdrgpu_{self._kind}_{name}")
 
     def __del__(self):
         try:
             if self._h:
-                self.ctx._lib.tsdrgpu_spectrum_destroy(self._h)
+                self._fn("destroy")(self._h)
                 self._h = None
         except Exception:
             pass
+
+    def reset(self) -> None:
+        """Discard the open segment and the report in progress."""
+        self.ctx.chk(self._fn("reset")(self._h))
+
+    def run(self, iq: torch.Tensor, discontinuity: bool = False) -> torch.Tensor:
+        """Interleaved float32 I,Q on the device (8-byte aligned) -> the reports this run completes, (R, N) float64 on the device in
+        fftshift order (asynchronous on the current stream).  discontinuity: these pairs do not follow the last run's."""
+        _f32(iq)
+        pairs = iq.numel() // 2
+        n = C.c_uint32(0)
+        self.ctx.chk(self._fn("plan")(self._h, pairs, int(discontinuity), C.byref(n)))
+        out = torch.empty((n.value, self.n), dtype=torch.float64, device=iq.device)
+        got = C.c_uint32(0)
+        self.ctx.chk(self._fn("run")(self._h, self.ctx.stream, iq.data_ptr(), pairs, int(discontinuity),
+                                     out.data_ptr() if n.value else None, n.value, C.byref(got)))
+        assert got.value == n.value
+        return out
+
+
+class Spectrum(_SegmentReports):
+    """The Welch power spectrum of tsdrgpu.h: windowed, 50 % overlapping segments of the IQ stream, K of them averaged per report,
+    with the open segment carried from run to run."""
+    _kind = "spectrum"
 
     def set(self, spec: str, samplerate: int) -> None:
         """"welch:<N>[:<rate>]" at `samplerate` from the next run on; a new spec or rate starts a new report."""
@@ -299,24 +326,6 @@ class Spectrum:
             raise ValueError("Spectrum.set needs a 'welch:...' spec")
         self.ctx.chk(self.ctx._lib.tsdrgpu_spectrum_set(self._h, C.byref(s), samplerate))
         self.n = s.n
-
-    def reset(self) -> None:
-        """Discard the open segment and the report in progress."""
-        self.ctx.chk(self.ctx._lib.tsdrgpu_spectrum_reset(self._h))
-
-    def run(self, iq: torch.Tensor, discontinuity: bool = False) -> torch.Tensor:
-        """Interleaved float32 I,Q on the device (8-byte aligned) -> the reports this run completes, (R, N) float64 on the device in
-        fftshift order (asynchronous on the current stream).  discontinuity: these pairs do not follow the last run's."""
-        _f32(iq)
-        pairs = iq.numel() // 2
-        n = C.c_uint32(0)
-        self.ctx.chk(self.ctx._lib.tsdrgpu_spectrum_plan(self._h, pairs, int(discontinuity), C.byref(n)))
-        out = torch.empty((n.value, self.n), dtype=torch.float64, device=iq.device)
-        got = C.c_uint32(0)
-        self.ctx.chk(self.ctx._lib.tsdrgpu_spectrum_run(self._h, self.ctx.stream, iq.data_ptr(), pairs, int(discontinuity),
-                                                        out.data_ptr() if n.value else None, n.value, C.byref(got)))
-        assert got.value == n.value
-        return out
 
     @staticmethod
     def window(n: int) -> np.ndarray:
@@ -331,24 +340,10 @@ class Spectrum:
         return N.lib().tsdrgpu_spectrum_k(C.byref(N.spectrum_spec(spec)), samplerate)
 
 
-class Coherence:
+class Coherence(_SegmentReports):
     """The spectral coherence at the line rate of tsdrgpu.h: each segment of the Welch spectrum's segmentation transformed with the
     complex windows w+ and w-, |sum U+ conj(U-) e^{-2 pi i alpha s/fs}| / sqrt(sum |U+|^2 sum |U-|^2) per report."""
-
-    def __init__(self, ctx: Context):
-        self.ctx = ctx
-        h = C.c_void_p()
-        ctx.chk(ctx._lib.tsdrgpu_coherence_create(ctx._h, C.byref(h)))
-        self._h = h
-        self.n = 0
-
-    def __del__(self):
-        try:
-            if self._h:
-                self.ctx._lib.tsdrgpu_coherence_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+    _kind = "coherence"
 
     def set(self, spec: str, samplerate: int, alpha: float) -> None:
         """"line[:<rate>]" at `samplerate` and line rate `alpha` (Hz) from the next run on; alpha alone takes effect at the next
@@ -358,24 +353,6 @@ class Coherence:
             raise ValueError("Coherence.set needs a 'line...' spec")
         self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_set(self._h, C.byref(s), samplerate, float(alpha)))
         self.n = Coherence.n_for(samplerate, alpha)
-
-    def reset(self) -> None:
-        """Discard the open segment and the report in progress."""
-        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_reset(self._h))
-
-    def run(self, iq: torch.Tensor, discontinuity: bool = False) -> torch.Tensor:
-        """Interleaved float32 I,Q on the device (8-byte aligned) -> the reports this run completes, (R, N) float64 on the device in
-        fftshift order (asynchronous on the current stream).  discontinuity: these pairs do not follow the last run's."""
-        _f32(iq)
-        pairs = iq.numel() // 2
-        n = C.c_uint32(0)
-        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_plan(self._h, pairs, int(discontinuity), C.byref(n)))
-        out = torch.empty((n.value, self.n), dtype=torch.float64, device=iq.device)
-        got = C.c_uint32(0)
-        self.ctx.chk(self.ctx._lib.tsdrgpu_coherence_run(self._h, self.ctx.stream, iq.data_ptr(), pairs, int(discontinuity),
-                                                         out.data_ptr() if n.value else None, n.value, C.byref(got)))
-        assert got.value == n.value
-        return out
 
     @staticmethod
     def n_for(samplerate: int, alpha: float) -> int:

@@ -1596,23 +1596,26 @@ int acc_ctas_per_sm(int log2L, int threads, size_t smem, bool pair) {
 }  // namespace
 
 // The segmentation the Welch spectrum and the coherence share: segments of N pairs with hop N/2, the open segment (fewer than N
-// pairs) carried across runs in d_hist, and reports of K segments.  seg_run hands the completed segments of a run to `launch` in
-// pieces of at most seg_chunk segments (all of them: 0) that stay inside one report, over at most rows_max rows of partial sums, and
-// calls `finish` for every report completed.
+// pairs) carried across runs in d_hist, and reports of K segments, each segment taken as per_seg transforms and summed into `planes`
+// planes of N partial sums.  seg_run hands the completed segments of a run to `launch` in pieces of at most seg_chunk segments (all
+// of them: 0) that stay inside one report, over at most rows_max rows of partial sums, and calls `finish` for every report completed.
 struct SegStream {
 	uint32_t N, K;                                // N == 0: no spec set yet
+	unsigned per_seg, planes;                     // 1, 1: the spectrum; 2, 4: the coherence (fft_acc2_kernel)
+	bool break_report;                            // a discontinuity also discards the report in progress
+	int stale;                                    // the device buffers are not those of N yet: the next run (re)builds them
 	DeviceBuf<float> d_hist, d_join;              // the open segment; the open segment followed by the head of a block
+	DeviceBuf<double> d_acc;                      // rows_max rows of `planes` x N partial sums of the report in progress
+	DeviceBuf<float2> d_scratch;                  // two-pass plans: the first pass's output for seg_chunk segments
 	uint64_t open;                                // pairs of the open segment (in d_hist, fewer than N)
 	uint64_t done;                                // completed segments of the report in progress (< K)
 	unsigned rows_used, rows_max, seg_chunk;      // rows of partial sums that hold sums of the report in progress
 	void reset() { open = 0; done = 0; rows_used = 0; }
-	// reports the next run would complete; break_report: a discontinuity also discards the report in progress
-	uint32_t plan(uint64_t pairs, int discontinuity, bool break_report) const {
+	// reports the next run would complete
+	uint32_t plan(uint64_t pairs, int discontinuity) const {
 		const uint64_t total = (discontinuity ? 0 : open) + pairs, count = total >= N ? (total - N) / (N / 2) + 1 : 0;
 		return (uint32_t) (((discontinuity && break_report ? 0 : done) + count) / K);
 	}
-	// the history buffers of N, once the work that used the old ones on `stream` is done (the caller has synchronised it)
-	cudaError_t build() { cudaError_t e = d_hist.assign(2 * (size_t) N); return e == cudaSuccess ? d_join.assign(4 * (size_t) N) : e; }
 };
 
 // launch(src, first, n, rows, keep): n consecutive segments from src (pairs, N/2 apart), segments first .. first + n - 1 of the
@@ -1622,7 +1625,7 @@ int seg_run(tsdrgpu_ctx_t *ctx, SegStream &g, cudaStream_t stream, const float *
             Finish finish, uint32_t *h_nreports) {
 	int rc;
 	*h_nreports = 0;
-	if (discontinuity) g.open = 0;
+	if (discontinuity) { if (g.break_report) g.reset(); else g.open = 0; }
 	if (pairs == 0) return TSDRGPU_OK;
 	const uint64_t N = g.N, H = N / 2, L = g.open, total = L + pairs;
 	const uint64_t count = total >= N ? (total - N) / H + 1 : 0;        // segments completed by this run, q = 0 .. count-1
@@ -1659,17 +1662,57 @@ int seg_run(tsdrgpu_ctx_t *ctx, SegStream &g, cudaStream_t stream, const float *
 	return TSDRGPU_OK;
 }
 
+// the device buffers of N, once the work that used the old ones on `stream` is done: rows_max rows of partial sums, one CTA per row
+// and bundle of the accumulating last pass at its occupancy, and the two-pass plans' scratch for seg_chunk segments
+int seg_build(tsdrgpu_ctx_t *ctx, SegStream &g, cudaStream_t stream) {
+	const AccShape a = acc_shape(ilog2(g.N));
+	{ std::lock_guard<std::mutex> lock(ctx->mu); if (const int rc = pass_attrs(ctx)) return rc; }     // the occupancy below depends on it
+	const unsigned ctas = (unsigned) acc_ctas_per_sm(a.log2L, a.threads, a.smem, g.per_seg == 2) * (unsigned) ctx->sm_count;
+	const unsigned long long NP = (unsigned long long) g.N * g.per_seg;
+	g.rows_max = ctas / a.bundles > 0 ? ctas / a.bundles : 1;
+	g.seg_chunk = ilog2(g.N) <= (unsigned) FFT_MAX_LOG2L ? 0u : (unsigned) (SP_SCRATCH_POINTS / NP > 0 ? SP_SCRATCH_POINTS / NP : 1);
+	CU_TRY(ctx, cudaStreamSynchronize(stream));
+	CU_TRY(ctx, g.d_hist.assign(2 * (size_t) g.N));
+	CU_TRY(ctx, g.d_join.assign(4 * (size_t) g.N));
+	CU_TRY(ctx, g.d_acc.assign((size_t) g.rows_max * g.planes * g.N));
+	if (g.seg_chunk) CU_TRY(ctx, g.d_scratch.assign((size_t) g.seg_chunk * NP));
+	return TSDRGPU_OK;
+}
+
+// The preamble of both runs: the arguments, the reports the run completes against the output's capacity (`what` names the run in
+// the errors), and when stale the buffers of N rebuilt once the work that used the old ones on `stream` is done, `window` putting
+// the caller's window in place.
+template <class Window>
+int seg_begin(tsdrgpu_ctx_t *ctx, const char *what, SegStream &g, cudaStream_t stream, const float *d_iq, uint64_t pairs,
+              int discontinuity, const double *d_reports, uint32_t capacity, uint32_t *h_nreports, Window window) {
+	char msg[80];
+	if (g.N == 0) {
+		snprintf(msg, sizeof msg, "%s run before a spec was set", what);
+		return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, msg, cudaSuccess, __FILE__, __LINE__);
+	}
+	ARG_TRY(ctx, h_nreports != NULL && pairs <= (1ull << 40));
+	ARG_TRY(ctx, pairs == 0 || (d_iq != NULL && ((uintptr_t) d_iq & 7u) == 0));
+	const uint32_t nrep = g.plan(pairs, discontinuity);
+	if (nrep > capacity) {
+		snprintf(msg, sizeof msg, "%s run: more reports than the output holds", what);
+		return tsdrgpu_fail(ctx, TSDRGPU_ECAPACITY, msg, cudaSuccess, __FILE__, __LINE__);
+	}
+	ARG_TRY(ctx, nrep == 0 || d_reports != NULL);
+	if (!g.stale) return TSDRGPU_OK;
+	int rc;
+	if ((rc = seg_build(ctx, g, stream)) || (rc = window())) return rc;
+	g.stale = 0;
+	return TSDRGPU_OK;
+}
+
 struct tsdrgpu_spectrum {
 	tsdrgpu_ctx_t *ctx;
 	tsdrgpu_welch_t spec;                         // n == 0: no spec set yet
 	uint32_t fs;
 	double scale;                                 // 1 / (K (sum w)^2)
 	std::vector<float> h_win;                     // the float32 window of spec.n
-	int stale;                                    // the device buffers are not those of spec.n yet: the next run (re)builds them
 	SegStream seg;                                // N = spec.n, K
 	DeviceBuf<float> d_win;                       // the window
-	DeviceBuf<double> d_acc;                      // rows_max rows of N partial sums of the report in progress
-	DeviceBuf<float2> d_scratch;                  // two-pass plans: the first pass's output for seg_chunk segments
 };
 
 extern "C" {
@@ -1677,7 +1720,7 @@ extern "C" {
 int tsdrgpu_spectrum_create(tsdrgpu_ctx_t *ctx, tsdrgpu_spectrum_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
 	tsdrgpu_spectrum *s = new tsdrgpu_spectrum();      // value-initialised; buffers are sized by the first run after a set
-	s->ctx = ctx;
+	s->ctx = ctx; s->seg.per_seg = 1; s->seg.planes = 1;
 	*out = s;
 	return TSDRGPU_OK;
 }
@@ -1707,7 +1750,7 @@ int tsdrgpu_spectrum_set(tsdrgpu_spectrum_t *s, const tsdrgpu_welch_t *spec, uin
 		double sum = 0.0;
 		for (size_t i = 0; i < w.size(); i++) { s->h_win[i] = (float) w[i]; sum += (double) s->h_win[i]; }
 		s->scale = 1.0 / (sum * sum);
-		s->stale = 1;
+		s->seg.stale = 1;
 	} else s->scale *= (double) s->seg.K;
 	s->scale /= (double) K;
 	s->spec = *spec; s->fs = fs; s->seg.N = (uint32_t) spec->n; s->seg.K = K;
@@ -1716,39 +1759,9 @@ int tsdrgpu_spectrum_set(tsdrgpu_spectrum_t *s, const tsdrgpu_welch_t *spec, uin
 
 int tsdrgpu_spectrum_plan(const tsdrgpu_spectrum_t *s, uint64_t pairs, int discontinuity, uint32_t *nreports) {
 	if (!s || !nreports || s->spec.n == 0) return TSDRGPU_EINVAL;
-	*nreports = s->seg.plan(pairs, discontinuity, false);
+	*nreports = s->seg.plan(pairs, discontinuity);
 	return TSDRGPU_OK;
 }
-
-}  // extern "C"
-
-// rows_max and seg_chunk of an N-point plan whose last pass is `acc_kernel_ctas` CTAs per SM and whose first pass writes
-// `per_seg` transforms per segment to the scratch
-static void seg_shape(tsdrgpu_ctx_t *ctx, SegStream &g, int ctas_per_sm, unsigned bundles, unsigned per_seg) {
-	const unsigned ctas = (unsigned) ctas_per_sm * (unsigned) ctx->sm_count;
-	const unsigned long long NP = (unsigned long long) g.N * per_seg;
-	g.rows_max = ctas / bundles > 0 ? ctas / bundles : 1;
-	g.seg_chunk = ilog2(g.N) <= (unsigned) FFT_MAX_LOG2L ? 0u : (unsigned) (SP_SCRATCH_POINTS / NP > 0 ? SP_SCRATCH_POINTS / NP : 1);
-}
-
-// the device buffers of spec.n, once the work that used the old ones on `stream` is done
-static int spectrum_build(tsdrgpu_spectrum *s, cudaStream_t stream) {
-	tsdrgpu_ctx_t *ctx = s->ctx;
-	const size_t N = (size_t) s->spec.n;
-	const AccShape a = acc_shape(ilog2(N));
-	{ std::lock_guard<std::mutex> lock(ctx->mu); if (const int rc = pass_attrs(ctx)) return rc; }     // the occupancy below depends on it
-	seg_shape(ctx, s->seg, acc_ctas_per_sm(a.log2L, a.threads, a.smem, false), a.bundles, 1);
-	CU_TRY(ctx, cudaStreamSynchronize(stream));
-	CU_TRY(ctx, s->d_win.assign(N));
-	CU_TRY(ctx, s->seg.build());
-	CU_TRY(ctx, s->d_acc.assign((size_t) s->seg.rows_max * N));
-	if (s->seg.seg_chunk) CU_TRY(ctx, s->d_scratch.assign((size_t) s->seg.seg_chunk * N));
-	CU_TRY(ctx, cudaMemcpyAsync(s->d_win.ptr, s->h_win.data(), sizeof(float) * N, cudaMemcpyHostToDevice, stream));
-	s->stale = 0;
-	return TSDRGPU_OK;
-}
-
-extern "C" {
 
 int tsdrgpu_spectrum_run(tsdrgpu_spectrum_t *s, void *stream_, const float *d_iq, uint64_t pairs, int discontinuity,
                          double *d_reports, uint32_t capacity, uint32_t *h_nreports) {
@@ -1756,27 +1769,24 @@ int tsdrgpu_spectrum_run(tsdrgpu_spectrum_t *s, void *stream_, const float *d_iq
 	tsdrgpu_ctx_t *ctx = s->ctx;
 	BIND(ctx);
 	cudaStream_t stream = (cudaStream_t) stream_;
-	if (s->spec.n == 0) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "spectrum run before a spec was set", cudaSuccess, __FILE__, __LINE__);
-	ARG_TRY(ctx, h_nreports != NULL && pairs <= (1ull << 40));
-	ARG_TRY(ctx, pairs == 0 || (d_iq != NULL && ((uintptr_t) d_iq & 7u) == 0));
-	uint32_t nrep = 0;
-	tsdrgpu_spectrum_plan(s, pairs, discontinuity, &nrep);
-	if (nrep > capacity) return tsdrgpu_fail(ctx, TSDRGPU_ECAPACITY, "spectrum run: more reports than the output holds", cudaSuccess, __FILE__, __LINE__);
-	ARG_TRY(ctx, nrep == 0 || d_reports != NULL);
-	int rc;
-	if (s->stale && (rc = spectrum_build(s, stream))) return rc;
-	const unsigned long long N = (unsigned long long) s->spec.n;
+	const unsigned long long N = s->seg.N;
+	const int rc = seg_begin(ctx, "spectrum", s->seg, stream, d_iq, pairs, discontinuity, d_reports, capacity, h_nreports, [&]() -> int {
+		CU_TRY(ctx, s->d_win.assign(N));
+		CU_TRY(ctx, cudaMemcpyAsync(s->d_win.ptr, s->h_win.data(), sizeof(float) * N, cudaMemcpyHostToDevice, stream));
+		return TSDRGPU_OK;
+	});
+	if (rc) return rc;
 	auto launch = [&](const float *src, uint64_t, unsigned nq, unsigned rows, unsigned keep) -> int {
 		FftOpts o; memset(&o, 0, sizeof o);
 		o.scale = 1.0f; o.batch = nq; o.exact = true; o.win = s->d_win.ptr;
 		o.pair_in = src; o.pair_bs = (long long) N;
 		o.scratch_bs = (long long) N;
-		o.acc = s->d_acc.ptr; o.acc_bs = (long long) N; o.acc_rows = rows; o.acc_keep = keep;
-		return fft_run(ctx, stream, NULL, s->d_scratch.ptr, ilog2(N), 0, o);
+		o.acc = s->seg.d_acc.ptr; o.acc_bs = (long long) N; o.acc_rows = rows; o.acc_keep = keep;
+		return fft_run(ctx, stream, NULL, s->seg.d_scratch.ptr, ilog2(N), 0, o);
 	};
 	auto finish = [&](uint32_t r) -> int {
 		KL(ctx, "k_spectrum_finish", stream, k_spectrum_finish<<<grid1d(N, ctx->sm_count), 256, 0, stream>>>(
-			s->d_acc.ptr, (long long) N, s->seg.rows_used, (unsigned) N, s->scale, d_reports + (size_t) r * N));
+			s->seg.d_acc.ptr, (long long) N, s->seg.rows_used, (unsigned) N, s->scale, d_reports + (size_t) r * N));
 		return TSDRGPU_OK;
 	};
 	return seg_run(ctx, s->seg, stream, d_iq, pairs, discontinuity, launch, finish, h_nreports);
@@ -1813,11 +1823,8 @@ struct tsdrgpu_coherence {
 	uint32_t fs;
 	double alpha;                                 // the last set's; the report in progress uses alpha_rep
 	double alpha_rep;                             // the alpha whose window is in d_cwin (0: none yet)
-	int stale;                                    // the device buffers are not those of seg.N yet: the next run (re)builds them
-	SegStream seg;
+	SegStream seg;                                // planes of partial sums: Re C, Im C, P+, P-
 	DeviceBuf<float2> d_cwin;                     // w+ of alpha_rep
-	DeviceBuf<double> d_acc;                      // rows_max rows of 4 N partial sums (Re C, Im C, P+, P-) of the report in progress
-	DeviceBuf<float2> d_scratch;                  // two-pass plans: the first pass's output for seg_chunk segments (2 transforms each)
 	std::vector<float2> h_cwin;
 };
 
@@ -1826,7 +1833,8 @@ extern "C" {
 int tsdrgpu_coherence_create(tsdrgpu_ctx_t *ctx, tsdrgpu_coherence_obj_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
 	tsdrgpu_coherence *c = new tsdrgpu_coherence();    // value-initialised; buffers are sized by the first run after a set
-	c->ctx = ctx;
+	c->ctx = ctx; c->seg.per_seg = 2; c->seg.planes = 4;
+	c->seg.break_report = true;                        // the time reference of the report is lost with the run
 	*out = c;
 	return TSDRGPU_OK;
 }
@@ -1852,7 +1860,7 @@ int tsdrgpu_coherence_set(tsdrgpu_coherence_obj_t *c, const tsdrgpu_coherence_t 
 	if (K == 0) return tsdrgpu_fail(c->ctx, TSDRGPU_EINVAL, "invalid coherence spec, sample rate or line rate (tsdrgpu.h)", cudaSuccess, __FILE__, __LINE__);
 	c->alpha = alpha;                             // alone: from the next report on
 	if (spec->rate == c->spec.rate && fs == c->fs && N == c->seg.N) return TSDRGPU_OK;
-	if (N != c->seg.N) c->stale = 1;
+	if (N != c->seg.N) c->seg.stale = 1;
 	c->alpha_rep = 0;                             // the window depends on fs: rebuilt at the next report
 	c->spec = *spec; c->fs = fs; c->seg.N = N; c->seg.K = K;
 	return tsdrgpu_coherence_reset(c);
@@ -1860,29 +1868,9 @@ int tsdrgpu_coherence_set(tsdrgpu_coherence_obj_t *c, const tsdrgpu_coherence_t 
 
 int tsdrgpu_coherence_plan(const tsdrgpu_coherence_obj_t *c, uint64_t pairs, int discontinuity, uint32_t *nreports) {
 	if (!c || !nreports || c->spec.rate == 0) return TSDRGPU_EINVAL;
-	*nreports = c->seg.plan(pairs, discontinuity, true);
+	*nreports = c->seg.plan(pairs, discontinuity);
 	return TSDRGPU_OK;
 }
-
-}  // extern "C"
-
-static int coherence_build(tsdrgpu_coherence *c, cudaStream_t stream) {
-	tsdrgpu_ctx_t *ctx = c->ctx;
-	const size_t N = c->seg.N;
-	const AccShape a = acc_shape(ilog2(N));
-	{ std::lock_guard<std::mutex> lock(ctx->mu); if (const int rc = pass_attrs(ctx)) return rc; }
-	seg_shape(ctx, c->seg, acc_ctas_per_sm(a.log2L, a.threads, a.smem, true), a.bundles, 2);
-	CU_TRY(ctx, cudaStreamSynchronize(stream));
-	CU_TRY(ctx, c->d_cwin.assign(N));
-	CU_TRY(ctx, c->seg.build());
-	CU_TRY(ctx, c->d_acc.assign((size_t) c->seg.rows_max * 4 * N));
-	if (c->seg.seg_chunk) CU_TRY(ctx, c->d_scratch.assign((size_t) c->seg.seg_chunk * 2 * N));
-	c->alpha_rep = 0;
-	c->stale = 0;
-	return TSDRGPU_OK;
-}
-
-extern "C" {
 
 int tsdrgpu_coherence_run(tsdrgpu_coherence_obj_t *c, void *stream_, const float *d_iq, uint64_t pairs, int discontinuity,
                           double *d_reports, uint32_t capacity, uint32_t *h_nreports) {
@@ -1890,17 +1878,13 @@ int tsdrgpu_coherence_run(tsdrgpu_coherence_obj_t *c, void *stream_, const float
 	tsdrgpu_ctx_t *ctx = c->ctx;
 	BIND(ctx);
 	cudaStream_t stream = (cudaStream_t) stream_;
-	if (c->spec.rate == 0) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "coherence run before a spec was set", cudaSuccess, __FILE__, __LINE__);
-	ARG_TRY(ctx, h_nreports != NULL && pairs <= (1ull << 40));
-	ARG_TRY(ctx, pairs == 0 || (d_iq != NULL && ((uintptr_t) d_iq & 7u) == 0));
-	uint32_t nrep = 0;
-	tsdrgpu_coherence_plan(c, pairs, discontinuity, &nrep);
-	if (nrep > capacity) return tsdrgpu_fail(ctx, TSDRGPU_ECAPACITY, "coherence run: more reports than the output holds", cudaSuccess, __FILE__, __LINE__);
-	ARG_TRY(ctx, nrep == 0 || d_reports != NULL);
-	int rc;
-	if (c->stale && (rc = coherence_build(c, stream))) return rc;
-	if (discontinuity) { c->seg.done = 0; c->seg.rows_used = 0; }      // the time reference of the report is lost with the run
 	const unsigned long long N = c->seg.N;
+	const int rc = seg_begin(ctx, "coherence", c->seg, stream, d_iq, pairs, discontinuity, d_reports, capacity, h_nreports, [&]() -> int {
+		CU_TRY(ctx, c->d_cwin.assign(N));
+		c->alpha_rep = 0;                                               // uploaded at the next report's first segment
+		return TSDRGPU_OK;
+	});
+	if (rc) return rc;
 	auto launch = [&](const float *src, uint64_t first, unsigned nq, unsigned rows, unsigned keep) -> int {
 		if (first == 0 && c->alpha_rep != c->alpha) {                   // alpha is read at the first segment of a report
 			std::vector<double> w2(2 * N);
@@ -1915,13 +1899,13 @@ int tsdrgpu_coherence_run(tsdrgpu_coherence_obj_t *c, void *stream_, const float
 		o.scale = 1.0f; o.batch = 2 * nq; o.exact = true; o.cwin = c->d_cwin.ptr;
 		o.pair_in = src; o.pair_bs = (long long) N;
 		o.scratch_bs = (long long) N;
-		o.acc = c->d_acc.ptr; o.acc_bs = 4 * (long long) N; o.acc_rows = rows; o.acc_keep = keep;
+		o.acc = c->seg.d_acc.ptr; o.acc_bs = 4 * (long long) N; o.acc_rows = rows; o.acc_keep = keep;
 		o.coh.alpha = c->alpha_rep; o.coh.fs = (double) c->fs; o.coh.seg0 = first; o.coh.hop = N / 2; o.coh.plane = (long long) N;
-		return fft_run(ctx, stream, NULL, c->d_scratch.ptr, ilog2(N), 0, o);
+		return fft_run(ctx, stream, NULL, c->seg.d_scratch.ptr, ilog2(N), 0, o);
 	};
 	auto finish = [&](uint32_t r) -> int {
 		KL(ctx, "k_coherence_finish", stream, k_coherence_finish<<<grid1d(N, ctx->sm_count), 256, 0, stream>>>(
-			c->d_acc.ptr, 4 * (long long) N, c->seg.rows_used, (unsigned) N, d_reports + (size_t) r * N));
+			c->seg.d_acc.ptr, 4 * (long long) N, c->seg.rows_used, (unsigned) N, d_reports + (size_t) r * N));
 		return TSDRGPU_OK;
 	};
 	return seg_run(ctx, c->seg, stream, d_iq, pairs, discontinuity, launch, finish, h_nreports);

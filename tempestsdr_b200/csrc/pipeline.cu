@@ -20,9 +20,10 @@
 #include "common.cuh"
 #include "host_plan.h"
 #include <math.h>
-#include <pthread.h>
+#include <condition_variable>
 #include <deque>
 #include <memory>
+#include <thread>
 #include <vector>
 
 struct tsdrgpu_frd;
@@ -32,13 +33,30 @@ struct tsdrgpu_framestage;
 namespace {
 
 constexpr int PL_SLOTS = 4;
+using Stats = tsdrgpu_pipeline_stats_t;
+
+// The busy flags of one kind of delivery slot, under tsdrgpu_pipeline::mu.  The worker takes a slot before it queues a copy into
+// the slot's page-locked buffers; the delivery thread releases it once the job's callbacks have returned.
+struct SlotPool {
+	tsdrgpu_pipeline *p; int n;                       // n <= PL_SLOTS slots
+	uint64_t Stats::*delivered, Stats::*skipped;      // count what release delivers / what acquire finds no slot for (null: nothing)
+	int busy[PL_SLOTS];
+	int free_slot() const { for (int k = 0; k < n; k++) if (!busy[k]) return k; return -1; }
+	template <class F> bool any(F f) const { for (int k = 0; k < n; k++) if (f(k)) return true; return false; }   // f(k) for some slot k
+	int acquire(bool wait, uint64_t count);           // a free slot, or -1; wait: until the delivery thread frees one
+	void release(int slot, uint64_t count);           // also counts the job delivered and wakes whoever waits for that
+};
+
+enum JobKind { JOB_FRAMES, JOB_PLOTS, JOB_REPORT };
 
 struct FrameJob {
-	int kind;                 // 0 = frames, 1 = plots, 2 = barrier, 3 = a spectrum report, 4 = a coherence report
-	int slot, nframes, w, h;
-	int spec_n;               // spectrum or coherence report: N
+	JobKind kind;
+	SlotPool *pool;           // the slot's pool, released after delivery
+	int slot; uint32_t samplerate;   // samplerate: plots and reports
+	int nframes, w, h;
+	int plot_id, report_n;    // a report: TSDRGPU_PLOT_ID_SPECTRUM or _COHERENCE, and N
+	double *report;           // a report: its values in the slot
 	cudaEvent_t ev;
-	uint32_t samplerate;      // plots
 	int foff, flen, loff, llen; uint64_t calls; int reset_announce, dump_announce;
 	int detect_mode;          // plots: announce the video mode detected from them
 	int snr_valid;            // frames: results carry an SNR to announce
@@ -146,6 +164,15 @@ struct SbRank {
 	~SbRank() { cudaSetDevice(dev); if (own.c) { if (stream) cudaStreamDestroy(stream); if (copy) cudaStreamDestroy(copy); if (ev) cudaEventDestroy(ev); } }
 };
 
+// A report side path (the Welch spectrum, the coherence): its object runs over every converted block on s_spec, and its reports go
+// out through slots of their own, so one path's reports waiting for delivery never take the other path's slots.
+template <class Obj> struct ReportPath {
+	int plot_id; SlotPool pool;
+	Obj *obj;                                          // created on first use
+	DeviceBuf<double> d_out; PinnedBuf<double> h[PL_SLOTS];
+	int fresh;                                         // blocks went by without this path: the next one starts a new report
+};
+
 struct tsdrgpu_pipeline {
 	tsdrgpu_ctx_t *ctx;
 	tsdrgpu_pipeline_config_t cfg;
@@ -176,14 +203,11 @@ struct tsdrgpu_pipeline {
 	// channel filter (tsdrgpu_pipeline_set_channel): created on first use
 	tsdrgpu_chanfilt *cf; DeviceBuf<float> d_cf_out;
 	int cf_stale;                                      // a block with samples went by unfiltered: zero the history before the next
-	// Welch spectrum (tsdrgpu_pipeline_set_spectrum): the object is created on first use, its work runs on s_spec (low priority)
-	tsdrgpu_spectrum *sp; cudaStream_t s_spec;
+	// Welch spectrum and coherence (tsdrgpu_pipeline_set_spectrum, _set_coherence): their work runs on s_spec (low priority)
+	ReportPath<tsdrgpu_spectrum> spec{TSDRGPU_PLOT_ID_SPECTRUM, {this, PL_SLOTS, &Stats::spectra_delivered, &Stats::spectra_skipped}};
+	ReportPath<tsdrgpu_coherence> coh{TSDRGPU_PLOT_ID_COHERENCE, {this, PL_SLOTS, &Stats::coherence_delivered, &Stats::coherence_skipped}};
+	cudaStream_t s_spec;
 	cudaEvent_t ev_conv, ev_sp_used[4];                // the block is converted / s_spec (spectrum, coherence) has read staging slot i
-	DeviceBuf<double> d_sp_out; PinnedBuf<double> h_spec[PL_SLOTS]; int spec_busy[PL_SLOTS];
-	int sp_fresh;                                      // blocks went by without the spectrum: the next one starts a new report
-	// coherence (tsdrgpu_pipeline_set_coherence): as the spectrum, on s_spec; ev_sp_used covers both readers of a staging slot
-	tsdrgpu_coherence *ch; DeviceBuf<double> d_ch_out; PinnedBuf<double> h_coh[PL_SLOTS]; int coh_busy[PL_SLOTS];
-	int ch_fresh;
 	DeviceBuf<float> d_pix; size_t pix_read, pix_fill;
 	DropComp pix_drop;
 	// stage 3: frames
@@ -196,10 +220,11 @@ struct tsdrgpu_pipeline {
 	double stack_ref; int stack_frames;
 	std::vector<double> h_pll_rr[PL_SLOTS];            // refresh rate after frame f when the PLL moved it there (NaN: it did not)
 	cudaEvent_t ev_res;                                // the batch's sync results have reached the host (PLL write-back needs them)
-	int slot_busy[PL_SLOTS];
+	SlotPool frame_slots{this, PL_SLOTS, &Stats::frames_delivered, &Stats::frames_dropped};
 	// autocorrelation side path
 	tsdrgpu_frd *frd; DeviceBuf<float> d_capture[2]; size_t cap_fill; int cap_phase; uint32_t cap_rate;
-	PinnedBuf<double> h_plot_frame[2], h_plot_line[2]; int plot_busy[2];
+	PinnedBuf<double> h_plot_frame[2], h_plot_line[2];
+	SlotPool plot_slots{this, 2, &Stats::plots_delivered, nullptr};
 	PinnedBuf<int32_t> h_peaks[2];                     // where the two plots peak, picked on the device (8f-3)
 	// superbandwidth (superb_run's state machine, superbandwidth.c:179-264)
 	struct {
@@ -211,12 +236,30 @@ struct tsdrgpu_pipeline {
 		tsdrgpu_superb_mgpu_t *grp[16];               // the sharded mode's group, one member per rank, once the hop size is known
 	} sb;
 	// delivery
-	pthread_t thread; pthread_mutex_t mu; pthread_cond_t cv_job, cv_done;
+	std::thread thread; std::mutex mu; std::condition_variable cv_job, cv_done;
 	std::deque<FrameJob> jobs; int stop; uint64_t submitted, delivered;
 	tsdrgpu_pipeline_stats_t stats;
 };
 
 enum { SB_STOPPED = 0, SB_STARTING, SB_GATHERING, SB_PAUSE };
+
+int SlotPool::acquire(bool wait, uint64_t count) {
+	std::unique_lock<std::mutex> g(p->mu);
+	int slot;
+	while ((slot = free_slot()) < 0 && wait) p->cv_done.wait(g);
+	if (slot >= 0) busy[slot] = 1; else if (skipped) p->stats.*skipped += count;
+	return slot;
+}
+void SlotPool::release(int slot, uint64_t count) {
+	std::lock_guard<std::mutex> g(p->mu);
+	busy[slot] = 0; p->stats.*delivered += count; p->delivered++;
+	p->cv_done.notify_all();
+}
+// every job submitted so far has been delivered: before a pool's page-locked buffers are regrown, and by flush
+static void wait_delivered(tsdrgpu_pipeline *p) {
+	std::unique_lock<std::mutex> g(p->mu);
+	while (p->delivered < p->submitted) p->cv_done.wait(g);
+}
 
 static void geometry(Settings &s) {                    // set_internal_samplerate, TSDRLibrary.c:540-550
 	double pr, pt; int w;
@@ -235,18 +278,17 @@ template <class F> static int update(tsdrgpu_pipeline *p, bool valid, F write) {
 	return TSDRGPU_OK;
 }
 
-static void *delivery_main(void *arg) {
-	tsdrgpu_pipeline *p = (tsdrgpu_pipeline *) arg;
+static void delivery_main(tsdrgpu_pipeline *p) {
 	cudaSetDevice(p->ctx->device);
 	tsdrgpu_bind_thread_near_device(p->ctx);          // the frames it hands out live in page-locked memory on the device's node
 	for (;;) {
-		pthread_mutex_lock(&p->mu);
-		while (p->jobs.empty() && !p->stop) pthread_cond_wait(&p->cv_job, &p->mu);
-		if (p->jobs.empty() && p->stop) { pthread_mutex_unlock(&p->mu); break; }
+		std::unique_lock<std::mutex> g(p->mu);
+		while (p->jobs.empty() && !p->stop) p->cv_job.wait(g);
+		if (p->jobs.empty()) break;                     // stopped, and every job delivered
 		FrameJob j = p->jobs.front(); p->jobs.pop_front();
-		pthread_mutex_unlock(&p->mu);
+		g.unlock();
 		cudaEventSynchronize(j.ev);
-		if (j.kind == 0) {
+		if (j.kind == JOB_FRAMES) {
 			const size_t n = (size_t) j.w * j.h;
 			for (int f = 0; f < j.nframes; f++) {
 				const tsdrgpu_frame_result_t &r = p->h_results[j.slot].ptr[f];
@@ -268,10 +310,7 @@ static void *delivery_main(void *arg) {
 				}
 				if (p->frame_cb) p->frame_cb(p->h_frames[j.slot].ptr + f * n, j.w, j.h, p->user);
 			}
-			pthread_mutex_lock(&p->mu);
-			p->slot_busy[j.slot] = 0; p->stats.frames_delivered += j.nframes;
-			pthread_mutex_unlock(&p->mu);
-		} else if (j.kind == 1) {
+		} else if (j.kind == JOB_PLOTS) {
 			if (j.reset_announce && p->value_cb) p->value_cb(1 /* VALUE_ID_AUTOCORRECT_RESET */, 0, 0, p->user);
 			if (j.dump_announce && p->value_cb) p->value_cb(5 /* VALUE_ID_AUTOCORRECT_DUMPED, frameratedetector.c:115 */, 0, 0, p->user);
 			if (p->plot_cb) {
@@ -284,37 +323,18 @@ static void *delivery_main(void *arg) {
 				tsdrgpu_detect_videomode(p->h_plot_frame[j.slot].ptr, j.foff, j.flen, p->h_plot_line[j.slot].ptr, j.loff, j.llen, j.samplerate, &fps, &height, NULL, NULL);
 				p->value_cb(TSDRGPU_VALUE_ID_DETECTED_MODE, fps, (double) height, p->user);
 			}
-			pthread_mutex_lock(&p->mu);
-			p->plot_busy[j.slot] = 0; p->stats.plots_delivered++;
-			pthread_mutex_unlock(&p->mu);
-		} else if (j.kind == 3) {
-			if (p->plot_cb) p->plot_cb(TSDRGPU_PLOT_ID_SPECTRUM, -j.spec_n / 2, p->h_spec[j.slot].ptr, j.spec_n, j.samplerate, p->user);
-			pthread_mutex_lock(&p->mu);
-			p->spec_busy[j.slot] = 0; p->stats.spectra_delivered++;
-			pthread_mutex_unlock(&p->mu);
-		} else if (j.kind == 4) {
-			if (p->plot_cb) p->plot_cb(TSDRGPU_PLOT_ID_COHERENCE, -j.spec_n / 2, p->h_coh[j.slot].ptr, j.spec_n, j.samplerate, p->user);
-			pthread_mutex_lock(&p->mu);
-			p->coh_busy[j.slot] = 0; p->stats.coherence_delivered++;
-			pthread_mutex_unlock(&p->mu);
-		}
+		} else if (p->plot_cb) p->plot_cb(j.plot_id, -j.report_n / 2, j.report, j.report_n, j.samplerate, p->user);
 		cudaEventDestroy(j.ev);
-		pthread_mutex_lock(&p->mu);
-		p->delivered++;
-		pthread_cond_broadcast(&p->cv_done);
-		pthread_mutex_unlock(&p->mu);
+		j.pool->release(j.slot, j.kind == JOB_FRAMES ? (uint64_t) j.nframes : 1);
 	}
-	return NULL;
 }
 
 static int submit(tsdrgpu_pipeline *p, FrameJob &j, cudaStream_t on) {
-	tsdrgpu_ctx_t *ctx = p->ctx;
-	CU_TRY(ctx, cudaEventCreateWithFlags(&j.ev, cudaEventDisableTiming));
-	CU_TRY(ctx, cudaEventRecord(j.ev, on));
-	pthread_mutex_lock(&p->mu);
+	CU_TRY(p->ctx, cudaEventCreateWithFlags(&j.ev, cudaEventDisableTiming));
+	CU_TRY(p->ctx, cudaEventRecord(j.ev, on));
+	std::lock_guard<std::mutex> g(p->mu);
 	p->jobs.push_back(j); p->submitted++;
-	pthread_cond_signal(&p->cv_job);
-	pthread_mutex_unlock(&p->mu);
+	p->cv_job.notify_one();
 	return TSDRGPU_OK;
 }
 
@@ -416,20 +436,13 @@ static int feed_capture(tsdrgpu_pipeline *p, const Settings &s, const float *d_i
 			int fmin, fmax, lmin, lmax;
 			tsdrgpu_frd_windows(s.samplerate, &fmin, &fmax, &lmin, &lmax);
 			const size_t need = (size_t) (fmax - fmin) + 8;
-			// pick a free plot slot; when the host is slower than the GPU the capture is still accumulated on
+			// a free plot slot; when the host is slower than the GPU the capture is still accumulated on
 			// the device, only this particular plot delivery is skipped
-			pthread_mutex_lock(&p->mu);
-			int slot = -1;
-			for (int k = 0; k < 2; k++) if (!p->plot_busy[k]) { slot = k; break; }
-			if (slot >= 0) p->plot_busy[slot] = 1;
-			pthread_mutex_unlock(&p->mu);
-			bool regrow = false;                                                // too small, or left empty by a failed re-allocation
-			for (int k = 0; k < 2; k++) regrow |= p->h_plot_frame[k].cap < need || p->h_plot_line[k].cap < need || !p->h_peaks[k].ptr;
-			if (regrow) {
+			const int slot = p->plot_slots.acquire(false, 1);
+			// too small, or left empty by a failed re-allocation
+			if (p->plot_slots.any([&](int k) { return p->h_plot_frame[k].cap < need || p->h_plot_line[k].cap < need || !p->h_peaks[k].ptr; })) {
 				CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
-				pthread_mutex_lock(&p->mu);
-				while (p->delivered < p->submitted) pthread_cond_wait(&p->cv_done, &p->mu);
-				pthread_mutex_unlock(&p->mu);
+				wait_delivered(p);
 				for (int k = 0; k < 2; k++) {
 					if ((rc = p->h_peaks[k].assign(ctx, 16))) return rc;
 					if ((rc = p->h_plot_frame[k].assign(ctx, need))) return rc;
@@ -449,8 +462,8 @@ static int feed_capture(tsdrgpu_pipeline *p, const Settings &s, const float *d_i
 			CU_TRY(ctx, cudaEventRecord(p->ev_cap_used[cph], p->s_main));
 			p->stats.captures++;
 			if (slot >= 0) {
-				FrameJob j; memset(&j, 0, sizeof j);
-				j.kind = 1; j.slot = slot; j.samplerate = s.samplerate; j.foff = fmin; j.flen = fmax - fmin; j.loff = lmin; j.llen = lmax - lmin;
+				FrameJob j{JOB_PLOTS, &p->plot_slots, slot, s.samplerate};
+				j.foff = fmin; j.flen = fmax - fmin; j.loff = lmin; j.llen = lmax - lmin;
 				j.calls = calls; j.reset_announce = reset_announce; j.dump_announce = dump_announce; j.detect_mode = s.detect_mode;
 				if ((rc = submit(p, j, p->s_main))) return rc;
 			}
@@ -469,28 +482,12 @@ static int drain_frames(tsdrgpu_pipeline *p, const Settings &s) {
 	while (p->pix_fill - p->pix_read >= n * (size_t) batch) {
 		const int nf = batch;
 		// a free delivery slot, or the batch is dropped whole (frames stay aligned), as a full ring would (circbuff.c:95-104)
-		pthread_mutex_lock(&p->mu);
-		int slot = -1;
-		for (int k = 0; k < PL_SLOTS; k++) if (!p->slot_busy[k]) { slot = k; break; }
-		if (slot >= 0) p->slot_busy[slot] = 1;
-		pthread_mutex_unlock(&p->mu);
-		if (slot < 0 && p->cfg.block_when_busy) {
-			pthread_mutex_lock(&p->mu);
-			while (slot < 0) {
-				for (int k = 0; k < PL_SLOTS; k++) if (!p->slot_busy[k]) { slot = k; break; }
-				if (slot < 0) pthread_cond_wait(&p->cv_done, &p->mu);
-			}
-			p->slot_busy[slot] = 1;
-			pthread_mutex_unlock(&p->mu);
-		}
-		if (slot < 0) { p->pix_read += n * nf; p->stats.frames_dropped += nf; continue; }
-		bool regrow = false;                                                   // too small, or left empty by a failed re-allocation
-		for (int k = 0; k < PL_SLOTS; k++) regrow |= p->h_frames[k].cap < n * nf || !p->h_results[k].ptr || !p->h_report[k].ptr || !p->h_stack[k].ptr;
-		if (regrow) {
+		const int slot = p->frame_slots.acquire(p->cfg.block_when_busy, (uint64_t) nf);
+		if (slot < 0) { p->pix_read += n * nf; continue; }
+		// too small, or left empty by a failed re-allocation
+		if (p->frame_slots.any([&](int k) { return p->h_frames[k].cap < n * nf || !p->h_results[k].ptr || !p->h_report[k].ptr || !p->h_stack[k].ptr; })) {
 			CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
-			pthread_mutex_lock(&p->mu);
-			while (p->delivered < p->submitted) pthread_cond_wait(&p->cv_done, &p->mu);
-			pthread_mutex_unlock(&p->mu);
+			wait_delivered(p);
 			for (int k = 0; k < PL_SLOTS; k++) {
 				p->h_pll_rr[k] = std::vector<double>(nf);
 				if ((rc = p->h_frames[k].assign(ctx, n * nf))) return rc;
@@ -536,8 +533,8 @@ static int drain_frames(tsdrgpu_pipeline *p, const Settings &s) {
 		p->stats.d2h_bytes += sizeof(float) * n * nf;
 		p->pix_read += n * nf;
 		p->stats.frames_processed += nf;
-		FrameJob j; memset(&j, 0, sizeof j);
-		j.kind = 0; j.slot = slot; j.nframes = nf; j.w = w; j.h = h; j.snr_valid = s.report_snr; j.pll_valid = pll_on; j.stack_valid = stack_on;
+		FrameJob j{JOB_FRAMES, &p->frame_slots, slot, 0, nf, w, h};
+		j.snr_valid = s.report_snr; j.pll_valid = pll_on; j.stack_valid = stack_on;
 		if (pll_on) {
 			// frameratepll's write-back (syncdetector.c:141-152).  The reference does it from its post-processing thread while the
 			// decimating thread reads refreshrate unlocked (SURVEY F9); here it is applied in stream order: the results of this
@@ -622,6 +619,36 @@ static int drain_blocks(tsdrgpu_pipeline *p) {
 	}
 }
 
+// One report path over a whole converted block on s_spec (after ev_conv), its reports queued for delivery in free slots of its pool.
+// N == 0 (a geometry the path cannot resolve): no reports, and a new one once it can.  set(obj): this block's settings.
+template <class Obj, class Create, class Reset, class Plan, class Run, class Set>
+static int report_block(tsdrgpu_pipeline *p, ReportPath<Obj> &r, size_t N, Create create, Reset reset, Plan plan, Run run, Set set,
+                        uint32_t samplerate, const float *stage, uint64_t pairs, bool dropped) {
+	tsdrgpu_ctx_t *ctx = p->ctx;
+	int rc;
+	if (N == 0) { r.fresh = 1; return TSDRGPU_OK; }
+	if (!r.obj && (rc = create(ctx, &r.obj))) return rc;
+	if ((rc = set(r.obj)) || (r.fresh && (rc = reset(r.obj)))) return rc;
+	r.fresh = 0;
+	uint32_t nrep = 0;
+	if ((rc = plan(r.obj, pairs, dropped, &nrep))) return rc;
+	CU_TRY(ctx, r.d_out.reserve(p->s_spec, nrep * N));              // grows behind s_spec's last use of the old buffer
+	if (nrep && r.pool.any([&](int k) { return r.h[k].cap < N; })) {        // too small, or left empty by a failed re-allocation
+		wait_delivered(p);
+		for (int k = 0; k < PL_SLOTS; k++) if ((rc = r.h[k].assign(ctx, N))) return rc;
+	}
+	if ((rc = run(r.obj, p->s_spec, stage, pairs, dropped, r.d_out.ptr, nrep, &nrep))) return rc;
+	for (uint32_t i = 0; i < nrep; i++) {
+		const int slot = r.pool.acquire(false, 1);
+		if (slot < 0) continue;
+		CU_TRY(ctx, cudaMemcpyAsync(r.h[slot].ptr, r.d_out.ptr + i * N, sizeof(double) * N, cudaMemcpyDeviceToHost, p->s_spec));
+		p->stats.d2h_bytes += sizeof(double) * N;
+		FrameJob j{JOB_REPORT, &r.pool, slot, samplerate, 0, 0, 0, r.plot_id, (int) N, r.h[slot].ptr};
+		if ((rc = submit(p, j, p->s_spec))) return rc;
+	}
+	return TSDRGPU_OK;
+}
+
 extern "C" {
 
 // the error a superbandwidth rank's own context holds (NULL: the thread's, where tsdrgpu_create leaves it), in the pipeline's
@@ -673,13 +700,12 @@ static int create_handles(tsdrgpu_pipeline *p) {
 // thread must not be running and the pipeline's device must be current.
 static void release(tsdrgpu_pipeline *p) {
 	tsdrgpu_resampler_destroy(p->rs); tsdrgpu_framestage_destroy(p->fs); tsdrgpu_frd_destroy(p->frd); tsdrgpu_chanfilt_destroy(p->cf);
-	tsdrgpu_spectrum_destroy(p->sp); tsdrgpu_coherence_destroy(p->ch);
+	tsdrgpu_spectrum_destroy(p->spec.obj); tsdrgpu_coherence_destroy(p->coh.obj);
 	for (auto &b : p->hostbufs) if (b.state == 1) { cudaHostUnregister(const_cast<void *>(b.base)); cudaGetLastError(); }
 	superb_release(p);
 	for (cudaStream_t *s : own_streams(p)) if (*s) cudaStreamDestroy(*s);
 	if (p->s_spec) cudaStreamDestroy(p->s_spec);
 	for (cudaEvent_t *e : own_events(p)) if (*e) cudaEventDestroy(*e);
-	pthread_mutex_destroy(&p->mu); pthread_cond_destroy(&p->cv_job); pthread_cond_destroy(&p->cv_done);
 	delete p;
 }
 
@@ -693,10 +719,9 @@ int tsdrgpu_pipeline_create(tsdrgpu_ctx_t *ctx, const tsdrgpu_pipeline_config_t 
 	s.samplerate = s.samplerate_real = cfg->samplerate; s.height = cfg->height; s.refreshrate = cfg->refreshrate; s.motionblur = cfg->motionblur;
 	memcpy(s.params, cfg->params_int, sizeof s.params);
 	geometry(s);
-	pthread_mutex_init(&p->mu, NULL); pthread_cond_init(&p->cv_job, NULL); pthread_cond_init(&p->cv_done, NULL);
 	const int rc = create_handles(p);
 	if (rc) { release(p); return rc; }
-	pthread_create(&p->thread, NULL, delivery_main, p);
+	p->thread = std::thread(delivery_main, p);
 	*out = p;
 	return TSDRGPU_OK;
 }
@@ -704,22 +729,16 @@ int tsdrgpu_pipeline_create(tsdrgpu_ctx_t *ctx, const tsdrgpu_pipeline_config_t 
 int tsdrgpu_pipeline_flush(tsdrgpu_pipeline_t *p) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, p != NULL);
 	BIND(p->ctx);
-	CU_TRY(p->ctx, cudaStreamSynchronize(p->s_copy));
-	CU_TRY(p->ctx, cudaStreamSynchronize(p->s_ingest));
-	CU_TRY(p->ctx, cudaStreamSynchronize(p->s_main));
-	CU_TRY(p->ctx, cudaStreamSynchronize(p->s_out));
-	CU_TRY(p->ctx, cudaStreamSynchronize(p->s_spec));
-	pthread_mutex_lock(&p->mu);
-	while (p->delivered < p->submitted) pthread_cond_wait(&p->cv_done, &p->mu);
-	pthread_mutex_unlock(&p->mu);
+	for (cudaStream_t st : {p->s_copy, p->s_ingest, p->s_main, p->s_out, p->s_spec}) CU_TRY(p->ctx, cudaStreamSynchronize(st));
+	wait_delivered(p);
 	return TSDRGPU_OK;
 }
 
 void tsdrgpu_pipeline_destroy(tsdrgpu_pipeline_t *p) {
 	if (!p) return;
 	tsdrgpu_pipeline_flush(p);
-	pthread_mutex_lock(&p->mu); p->stop = 1; pthread_cond_broadcast(&p->cv_job); pthread_mutex_unlock(&p->mu);
-	pthread_join(p->thread, NULL);
+	{ std::lock_guard<std::mutex> g(p->mu); p->stop = 1; p->cv_job.notify_all(); }
+	p->thread.join();
 	cudaSetDevice(p->ctx->device);
 	release(p);
 }
@@ -825,7 +844,7 @@ int tsdrgpu_pipeline_get_geometry(tsdrgpu_pipeline_t *p, int *width, int *height
 }
 int tsdrgpu_pipeline_stats(tsdrgpu_pipeline_t *p, tsdrgpu_pipeline_stats_t *out) {
 	if (!p || !out) return TSDRGPU_EINVAL;
-	pthread_mutex_lock(&p->mu); *out = p->stats; pthread_mutex_unlock(&p->mu);
+	{ std::lock_guard<std::mutex> g(p->mu); *out = p->stats; }
 	out->gpu_launches = p->ctx->launches;
 	return TSDRGPU_OK;
 }
@@ -1006,90 +1025,6 @@ static int channel_filter(tsdrgpu_pipeline *p, const tsdrgpu_channel_t *spec, ui
 	return tsdrgpu_chanfilt_run(p->cf, p->s_ingest, stage, pairs, p->d_cf_out.ptr);
 }
 
-// the spectrum over one whole converted block on s_spec (after ev_conv), its reports copied into free report slots and queued for
-// delivery
-static int spectrum_block(tsdrgpu_pipeline *p, const Settings &s, const float *stage, uint64_t pairs, bool dropped) {
-	tsdrgpu_ctx_t *ctx = p->ctx;
-	int rc;
-	if (!p->sp && (rc = tsdrgpu_spectrum_create(ctx, &p->sp))) return rc;
-	if ((rc = tsdrgpu_spectrum_set(p->sp, &s.sp_spec, s.samplerate))) return rc;          // a new spec or samplerate: a new report
-	if (p->sp_fresh && (rc = tsdrgpu_spectrum_reset(p->sp))) return rc;
-	p->sp_fresh = 0;
-	const size_t N = (size_t) s.sp_spec.n;
-	uint32_t nrep = 0;
-	if ((rc = tsdrgpu_spectrum_plan(p->sp, pairs, dropped, &nrep))) return rc;
-	if (p->d_sp_out.cap < nrep * N) {
-		CU_TRY(ctx, cudaStreamSynchronize(p->s_spec));
-		CU_TRY(ctx, p->d_sp_out.reserve(p->s_spec, nrep * N));
-	}
-	bool regrow = false;                                                    // too small, or left empty by a failed re-allocation
-	for (int k = 0; k < PL_SLOTS; k++) regrow |= p->h_spec[k].cap < N;
-	if (nrep && regrow) {
-		pthread_mutex_lock(&p->mu);
-		while (p->delivered < p->submitted) pthread_cond_wait(&p->cv_done, &p->mu);
-		pthread_mutex_unlock(&p->mu);
-		for (int k = 0; k < PL_SLOTS; k++) if ((rc = p->h_spec[k].assign(ctx, N))) return rc;
-	}
-	if ((rc = tsdrgpu_spectrum_run(p->sp, p->s_spec, stage, pairs, dropped, p->d_sp_out.ptr, nrep, &nrep))) return rc;
-	for (uint32_t r = 0; r < nrep; r++) {
-		pthread_mutex_lock(&p->mu);
-		int slot = -1;
-		for (int k = 0; k < PL_SLOTS; k++) if (!p->spec_busy[k]) { slot = k; break; }
-		if (slot >= 0) p->spec_busy[slot] = 1; else p->stats.spectra_skipped++;
-		pthread_mutex_unlock(&p->mu);
-		if (slot < 0) continue;
-		CU_TRY(ctx, cudaMemcpyAsync(p->h_spec[slot].ptr, p->d_sp_out.ptr + r * N, sizeof(double) * N, cudaMemcpyDeviceToHost, p->s_spec));
-		p->stats.d2h_bytes += sizeof(double) * N;
-		FrameJob j; memset(&j, 0, sizeof j);
-		j.kind = 3; j.slot = slot; j.spec_n = (int) N; j.samplerate = s.samplerate;
-		if ((rc = submit(p, j, p->s_spec))) return rc;
-	}
-	return TSDRGPU_OK;
-}
-
-// the coherence over one whole converted block on s_spec, as spectrum_block.  A geometry it cannot resolve makes no reports and
-// starts a new report once it can.
-static int coherence_block(tsdrgpu_pipeline *p, const Settings &s, const float *stage, uint64_t pairs, bool dropped) {
-	tsdrgpu_ctx_t *ctx = p->ctx;
-	int rc;
-	const double alpha = (double) s.height * s.refreshrate;
-	const size_t N = tsdrgpu_coherence_n(s.samplerate, alpha);
-	if (N == 0) { p->ch_fresh = 1; return TSDRGPU_OK; }
-	if (!p->ch && (rc = tsdrgpu_coherence_create(ctx, &p->ch))) return rc;
-	if ((rc = tsdrgpu_coherence_set(p->ch, &s.ch_spec, s.samplerate, alpha))) return rc;   // a new rate, fs or N: a new report
-	if (p->ch_fresh && (rc = tsdrgpu_coherence_reset(p->ch))) return rc;
-	p->ch_fresh = 0;
-	uint32_t nrep = 0;
-	if ((rc = tsdrgpu_coherence_plan(p->ch, pairs, dropped, &nrep))) return rc;
-	if (p->d_ch_out.cap < nrep * N) {
-		CU_TRY(ctx, cudaStreamSynchronize(p->s_spec));
-		CU_TRY(ctx, p->d_ch_out.reserve(p->s_spec, nrep * N));
-	}
-	bool regrow = false;
-	for (int k = 0; k < PL_SLOTS; k++) regrow |= p->h_coh[k].cap < N;
-	if (nrep && regrow) {
-		pthread_mutex_lock(&p->mu);
-		while (p->delivered < p->submitted) pthread_cond_wait(&p->cv_done, &p->mu);
-		pthread_mutex_unlock(&p->mu);
-		for (int k = 0; k < PL_SLOTS; k++) if ((rc = p->h_coh[k].assign(ctx, N))) return rc;
-	}
-	if ((rc = tsdrgpu_coherence_run(p->ch, p->s_spec, stage, pairs, dropped, p->d_ch_out.ptr, nrep, &nrep))) return rc;
-	for (uint32_t r = 0; r < nrep; r++) {
-		pthread_mutex_lock(&p->mu);
-		int slot = -1;
-		for (int k = 0; k < PL_SLOTS; k++) if (!p->coh_busy[k]) { slot = k; break; }
-		if (slot >= 0) p->coh_busy[slot] = 1; else p->stats.coherence_skipped++;
-		pthread_mutex_unlock(&p->mu);
-		if (slot < 0) continue;
-		CU_TRY(ctx, cudaMemcpyAsync(p->h_coh[slot].ptr, p->d_ch_out.ptr + r * N, sizeof(double) * N, cudaMemcpyDeviceToHost, p->s_spec));
-		p->stats.d2h_bytes += sizeof(double) * N;
-		FrameJob j; memset(&j, 0, sizeof j);
-		j.kind = 4; j.slot = slot; j.spec_n = (int) N; j.samplerate = s.samplerate;
-		if ((rc = submit(p, j, p->s_spec))) return rc;
-	}
-	return TSDRGPU_OK;
-}
-
 int tsdrgpu_pipeline_process(tsdrgpu_pipeline_t *p, const float *h_iq, uint64_t items_count, int64_t samples_dropped) {
 	return process_impl(p, h_iq, TSDRGPU_FMT_FLOAT, items_count, samples_dropped, true);
 }
@@ -1121,10 +1056,10 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 	const int w = s.width, h = s.height; const double ptos = s.ptos;     // the geometry at the call's start plans its blocks
 	p->stats.samples_in += size2;
 	if (samples_dropped > 0) p->stats.samples_dropped_upstream += (uint64_t) samples_dropped;
-	const bool sp_on = s.sp_spec.n != 0, ch_on = s.ch_spec.rate != 0;
-	if (s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION] || !sp_on) p->sp_fresh = 1;      // hops at other tunings, or no spectrum
-	if (s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION] || !ch_on) p->ch_fresh = 1;
-	if (s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION]) {
+	const bool sp_on = s.sp_spec.n != 0, ch_on = s.ch_spec.rate != 0, superres = s.params[TSDRGPU_PARAM_AUTOCORR_SUPERRESOLUTION] != 0;
+	p->spec.fresh |= superres || !sp_on;                                  // hops at other tunings, or the path is off
+	p->coh.fresh |= superres || !ch_on;
+	if (superres) {
 		if (size2 > 0) p->cf_stale = 1;                        // the hops are recorded unfiltered: the bands refer to one tuning
 		return superb_step(p, s, h_iq, fmt, items_count, samples_dropped);
 	}
@@ -1161,7 +1096,7 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 			if (fmt != TSDRGPU_FMT_FLOAT && (rc = raw_reserve(p, ss, bytes))) break;
 			const void *src = host_source(p, s.host_register, h_iq, bytes);
 			e = cudaStreamWaitEvent(p->s_copy, p->ev_used[ss], 0);
-			if (e == cudaSuccess && (p->sp || p->ch)) e = cudaStreamWaitEvent(p->s_copy, p->ev_sp_used[ss], 0);   // and s_spec's reads of it
+			if (e == cudaSuccess && (p->spec.obj || p->coh.obj)) e = cudaStreamWaitEvent(p->s_copy, p->ev_sp_used[ss], 0);   // and s_spec's reads of it
 			if (e == cudaSuccess) { e = cudaMemcpyAsync(fmt == TSDRGPU_FMT_FLOAT ? (void *) stage : p->d_raw[ss].ptr, src, bytes, cudaMemcpyHostToDevice, p->s_copy); copy_issued = true; }
 			if (e == cudaSuccess) e = cudaEventRecord(p->ev_h2d[ss], p->s_copy);
 			if (e == cudaSuccess) e = cudaStreamWaitEvent(p->s_ingest, p->ev_h2d[ss], 0);
@@ -1177,8 +1112,13 @@ static int process_impl(tsdrgpu_pipeline_t *p, const void *h_iq, int fmt, uint64
 				e = cudaEventRecord(p->ev_conv, fmt == TSDRGPU_FMT_FLOAT ? p->s_copy : p->s_ingest);
 				if (e == cudaSuccess) e = cudaStreamWaitEvent(p->s_spec, p->ev_conv, 0);
 				if (e != cudaSuccess) { rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "stream ordering", e, __FILE__, __LINE__); break; }
-				if (sp_on && (rc = spectrum_block(p, s, stage, size2, samples_dropped != 0))) break;
-				if (ch_on && (rc = coherence_block(p, s, stage, size2, samples_dropped != 0))) break;
+				if (sp_on && (rc = report_block(p, p->spec, (size_t) s.sp_spec.n, tsdrgpu_spectrum_create, tsdrgpu_spectrum_reset, tsdrgpu_spectrum_plan,
+				                                tsdrgpu_spectrum_run, [&](tsdrgpu_spectrum *o) { return tsdrgpu_spectrum_set(o, &s.sp_spec, s.samplerate); },
+				                                s.samplerate, stage, size2, samples_dropped != 0))) break;
+				const double alpha = (double) s.height * s.refreshrate;
+				if (ch_on && (rc = report_block(p, p->coh, (size_t) tsdrgpu_coherence_n(s.samplerate, alpha), tsdrgpu_coherence_create, tsdrgpu_coherence_reset,
+				                                tsdrgpu_coherence_plan, tsdrgpu_coherence_run, [&](tsdrgpu_coherence *o) { return tsdrgpu_coherence_set(o, &s.ch_spec, s.samplerate, alpha); },
+				                                s.samplerate, stage, size2, samples_dropped != 0))) break;
 				// ev_sp_used[ss] keeps the copy four calls later from overwriting the slot before s_spec has read it
 				if ((e = cudaEventRecord(p->ev_sp_used[ss], p->s_spec)) != cudaSuccess) { rc = tsdrgpu_fail(ctx, TSDRGPU_ECUDA, "stream ordering", e, __FILE__, __LINE__); break; }
 			}
