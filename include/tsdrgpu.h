@@ -624,8 +624,35 @@ TSDRGPU_API int  tsdrgpu_deblur(tsdrgpu_ctx_t *ctx, void *stream, const float *d
  * DESIGN.md section 5.5 gives the quality they were chosen for.  When no tile restarts, every m_t follows the global m's
  * sequence capped at N, so the output and records equal align's bit for bit; the record's `changed` counts the tiles restarted
  * in that frame (always 0 for align and on restart frames). */
-/* the stack's modes; any other value, 2 and 3 included, is refused with TSDRGPU_EINVAL */
-enum { TSDRGPU_STACK_OFF = 0, TSDRGPU_STACK_ALIGN = 1, TSDRGPU_STACK_ADAPT = 4 };
+/* The motion-tracking mode (TSDRGPU_STACK_TRACK, "track:<N>[:<rx>x<ry>]", the same ranges and defaults) carries the average
+ * tile by tile with content that moves inside the picture: a terminal that scrolls, a page scrolled in a browser, a window being
+ * dragged.  To adapt, every tile such motion crosses has changed, so the average restarts there at every move.  Here a changed
+ * tile first looks in the old average for where its content came from and, when it finds it, takes its average and counts
+ * from there; only what is newly exposed starts again.  Steps 1-5 and 7 are align's and 6a is adapt's, unchanged: D_t(0) = D_t,
+ * C_t(0) = C_t and changed_t against the tile's level e_t.  The counts are per pixel: c[p] <= N (16 bits), and A and c are
+ * double-buffered, since a moving tile gathers from other tiles' old values.  Pixel p = (X, Y), X = p mod W, Y = p div W.
+ *   6t. local search, only for tiles with changed_t (the tile's own flag, before the neighbour rule): for every integer
+ *      v = (vx, vy) != (0, 0) with |vx| <= LX = TSDRGPU_STACK_TRACK_LX and |vy| <= LY = TSDRGPU_STACK_TRACK_LY, over the tile's
+ *      pixels p whose four taps are valid and whose source s = (X - vx, Y - vy) lies inside the W x H raster (no wrap):
+ *      d = Q(x[p]) - Q(A[s]), D_t(v) = sum d^2 and C_t(v) = their count, exact integers.  v is admissible when C_t(v) > 0 and
+ *      2 C_t(v) >= C_t(0).  v* is the admissible v with the least D/C, compared as D(v) C(v') against D(v') C(v) exactly in
+ *      64 bits; ties go to the smaller |vx| + |vy|, then to the first in loop order (vy outer, vx inner, both ascending).
+ *      moved_t holds when v* exists and passes 6b's change test at the tile's own level: not (16 D(v*) > RATIO e_t C(v*) and
+ *      D(v*) > FLOOR C(v*)).
+ *   6b. a tile restarts when changed_t && !moved_t holds for it or one of its 8 neighbours (no wrap); a moved tile that a
+ *      neighbour restarts does restart; moved tiles do not spread restarts.
+ *   6c. a restarting tile takes e_t = none; a moved tile that does not restart takes r* = floor(16 D(v*) / C(v*)) and
+ *      e_t = floor((7 e_t + r*) / 8); every other tile follows adapt's 6c.
+ *   6d. blend into the second accumulator A' and counts c': the source is s = p - v* in a moved tile that does not restart and
+ *      s = p elsewhere; in a restarting tile, and for a pixel of a moved tile whose s falls outside the raster, s = p and c[s]
+ *      counts as 0.  k = min(c[s] + 1, N), with wn and wo from k as in align; A'[p] = A[s] wo + x[p] wn where all four taps
+ *      are valid, A'[p] = A[s] elsewhere; c'[p] = k in every case.  Then A' and c' are the state, and m += 1 as in align.
+ *   A restart frame sets every c = 1 and e_t = none; every restart of align restarts the counts, the levels and both planes.
+ * The record's `changed` counts the tiles restarted in the frame, as in adapt; tsdrgpu_stack_vectors reads where each tile
+ * moved.  LX and LY are fixed: 32 lines cover a one-line scroll of any usual font.  When no tile moves in a sequence, a tile's
+ * pixels share one count equal to adapt's m_t, so every output and record equals adapt's bit for bit. */
+/* the stack's modes; any other value, 2, 3 and 5 included, is refused with TSDRGPU_EINVAL */
+enum { TSDRGPU_STACK_OFF = 0, TSDRGPU_STACK_ALIGN = 1, TSDRGPU_STACK_ADAPT = 4, TSDRGPU_STACK_TRACK = 8 };
 #define TSDRGPU_STACK_MIN_N  2
 #define TSDRGPU_STACK_MAX_N  1024
 #define TSDRGPU_STACK_MAX_RX 32
@@ -633,15 +660,17 @@ enum { TSDRGPU_STACK_OFF = 0, TSDRGPU_STACK_ALIGN = 1, TSDRGPU_STACK_ADAPT = 4 }
 #define TSDRGPU_STACK_TILE   16
 #define TSDRGPU_STACK_ADAPT_RATIO 3
 #define TSDRGPU_STACK_ADAPT_FLOOR 64
+#define TSDRGPU_STACK_TRACK_LX 16
+#define TSDRGPU_STACK_TRACK_LY 32
 typedef struct {
 	double  offset;                               /* o (unwrapped; 0 on a restart frame) */
 	int64_t score;                                /* S(s*) (0 on a restart frame) */
 	int32_t dx, dy;                               /* the best candidate's place in the window */
 	int32_t restarted;                            /* 1 on a restart frame */
-	int32_t changed;                              /* adapt: the tiles restarted in this frame (0 for align) */
+	int32_t changed;                              /* adapt, track: the tiles restarted in this frame (0 for align) */
 } tsdrgpu_stack_record_t;
-/* host-only: the spelling shared by the host library's TSDR_STACK and Python.  "off", "align:<N>", "align:<N>:<rx>x<ry>",
- * "adapt:<N>" or "adapt:<N>:<rx>x<ry>"; N, rx, ry = one to six digits in the ranges above, rx and ry defaulting to 8 and 2.
+/* host-only: the spelling shared by the host library's TSDR_STACK and Python.  "off", "align:<N>", "align:<N>:<rx>x<ry>", and
+ * the same with "adapt:" or "track:"; N, rx, ry = one to six digits in the ranges above, rx and ry defaulting to 8 and 2.
  * Nothing else (no sign, blank or point).  TSDRGPU_OK with the four outputs set (zeros for "off"), else TSDRGPU_EINVAL and the
  * outputs untouched. */
 TSDRGPU_API int  tsdrgpu_stack_parse(const char *spec, int *mode, int *depth, int *rx, int *ry);
@@ -655,6 +684,11 @@ TSDRGPU_API int  tsdrgpu_stack_reset(tsdrgpu_stack_t *st);
 TSDRGPU_API int  tsdrgpu_stack_set(tsdrgpu_stack_t *st, int mode, int depth, int rx, int ry);
 TSDRGPU_API int  tsdrgpu_stack_run(tsdrgpu_stack_t *st, void *stream, const float *d_in, float *d_out, int w, int h, int nframes,
                                    tsdrgpu_stack_record_t *h_records_pinned);
+/* track mode (synchronises): where each tile of the last frame moved.  h_v receives 2 ntiles values, (vx, vy) of tile t at
+ * h_v[2t], h_v[2t + 1] with t = (Y div 16) ceil(W / 16) + X div 16: v* for a tile that moved and did not restart, (0, 0) (never a
+ * candidate) for every other tile and on a restart frame.  TSDRGPU_EINVAL unless the mode is track, a frame has been taken since
+ * the last restart and ntiles is the tile count of its geometry. */
+TSDRGPU_API int  tsdrgpu_stack_vectors(tsdrgpu_stack_t *st, int32_t *h_v, int ntiles);
 /* the frame stage's stack mode, applied from the next run on.  The mode is kept across tsdrgpu_framestage_reset; the accumulator
  * is not (the reset restarts it).  Out-of-range values or an unknown mode: TSDRGPU_EINVAL. */
 TSDRGPU_API int  tsdrgpu_framestage_set_stack(tsdrgpu_framestage_t *fs, int mode, int depth, int rx, int ry);
@@ -881,7 +915,7 @@ TSDRGPU_API int  tsdrgpu_pipeline_set_denoise(tsdrgpu_pipeline_t *p, int mode, i
 /* deblur mode (TSDRGPU_DEBLUR_OFF, the default, or TSDRGPU_DEBLUR_RL; see tsdrgpu_framestage_set_deblur), taking effect at the
  * next frame-stage batch */
 TSDRGPU_API int  tsdrgpu_pipeline_set_deblur(tsdrgpu_pipeline_t *p, int mode, int sigma_centi, int iterations);
-/* stack mode (TSDRGPU_STACK_OFF, the default, TSDRGPU_STACK_ALIGN or TSDRGPU_STACK_ADAPT; see tsdrgpu_framestage_set_stack),
+/* stack mode (TSDRGPU_STACK_OFF, the default, TSDRGPU_STACK_ALIGN, TSDRGPU_STACK_ADAPT or TSDRGPU_STACK_TRACK; see tsdrgpu_framestage_set_stack),
  * taking effect at the next frame-stage batch.  tsdrgpu_pipeline_sync restarts the stack at the next frame-stage batch.  While
  * the stack is on, every frame with an auto-gain report (dsp.c:231-235) also announces value id TSDRGPU_VALUE_ID_STACK_DRIFT with arg0 = the mean drift
  * in px/frame since the last announcement or restart ((o - o_last) / frames, 0 right after a restart) and arg1 = the frame's

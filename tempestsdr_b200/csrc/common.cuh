@@ -125,6 +125,13 @@ struct StackTile {
 	int flag;                                    // this frame: 0 no measured pixel (C_t = 0), 1 measured, 2 changed
 	float wo, wn;                                // this frame's blend weights
 };
+struct StackTrack {                              // track: one per tile of the accumulator, this frame's
+	int vx, vy;                                  // search: v* ((0, 0): no admissible candidate)
+	unsigned d, c;                               // search: D(v*), C(v*)
+	int moved;                                   // search: moved_t (meaningful where the tile's flag is 2)
+	int bx, by;                                  // decide: the move the blend takes, (0, 0) unless moved and not restarting
+	int restart;                                 // decide: the tile restarts
+};
 struct StackState {
 	int mode, depth, rx, ry;                     // TSDRGPU_STACK_* and its parameters (N, rx, ry)
 	int w, h;                                    // the accumulator's geometry
@@ -134,7 +141,10 @@ struct StackState {
 	DeviceBuf<double> d_off;                     // o1, o2
 	DeviceBuf<unsigned long long> d_scores;      // S of every candidate of the frame in flight
 	DeviceBuf<tsdrgpu_stack_record_t> d_rec;     // the records of a batch
-	DeviceBuf<StackTile> d_tiles;                // adapt: one per tile of the accumulator
+	DeviceBuf<StackTile> d_tiles;                // adapt, track: one per tile of the accumulator
+	DeviceBuf<float> d_acc2;                     // track: A', swapped with d_acc after every frame
+	DeviceBuf<uint16_t> d_cnt, d_cnt2;           // track: c and c', swapped likewise
+	DeviceBuf<StackTrack> d_track;               // track: one per tile of the accumulator
 };
 int stack_reserve(tsdrgpu_ctx_t *ctx, StackState *st, int nframes, int w, int h);
 int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h);

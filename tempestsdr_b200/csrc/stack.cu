@@ -3,10 +3,15 @@
 // partial scores, st_pick chooses s* and the sub-pixel offset and keeps the offsets on the device, st_blend warps the frame into
 // the accumulator and writes the output.  The adaptive mode replaces st_blend by three: st_tile_sums measures every tile's
 // residual and marks the changed ones, st_decide restarts them and their neighbours and sets each tile's weights, and
-// st_blend_tiles blends with those.  No host round trip inside a batch, and no CTA waits for another.  Built with -fmad=false;
+// st_blend_tiles blends with those.  The tracking mode keeps st_tile_sums and replaces the other two: st_track_search looks for
+// where each changed tile's content came from, st_track_decide restarts the tiles that changed and did not move (and their
+// neighbours), and st_track_blend gathers the accumulator and the per-pixel counts along each tile's move into the second
+// planes, which the host swaps with the first after every frame.  No host round trip inside a batch, and no CTA waits for another.  Built with -fmad=false;
 // the float arithmetic is spelled with __f*_rn anyway, so every output bit follows the definition.
 #include "common.cuh"
 #include "host_plan.h"
+
+#include <utility>
 
 namespace {
 
@@ -285,18 +290,190 @@ __global__ void __launch_bounds__(ST_THREADS) st_restart(const float *__restrict
 	}
 }
 
+// track, step 6t: one CTA per tile, returning at once unless the tile changed.  The CTA stages Q(x) of its tile (four pixels per
+// word, lowest byte first) with a byte mask of the pixels whose taps are valid, and the window of Q(A) every candidate reads:
+// (16 + 2 LX) x (16 + 2 LY) bytes, 0 outside the raster, one spare word per row so that byte_perm may read past the end.  Each
+// thread takes candidates in loop order; per word of the tile, byte_perm takes the candidate's horizontal phase, vabsdiffu4 the
+// distance, the mask the pixels of p and s both in the sum, and dp4a adds d^2 (D <= 256 * 255^2 < 2^32).  C(v) is the mask's
+// population.  The best candidate of a thread, of a warp and of the CTA, by the definition's exact order.
+constexpr int TK_LX = TSDRGPU_STACK_TRACK_LX, TK_LY = TSDRGPU_STACK_TRACK_LY;
+constexpr int TK_NX = 2 * TK_LX + 1, TK_NCAND = TK_NX * (2 * TK_LY + 1);
+constexpr int TK_WIN_ROWS = ST_TILE_PX + 2 * TK_LY;
+constexpr int TK_WIN_WORDS = (ST_TILE_PX + 2 * TK_LX) / 4 + 1;          // words per window row
+static_assert(TK_LX % 4 == 0 && ST_TILE_PX % 4 == 0, "window rows start on a word");
+struct TrackBest { unsigned d, c; int l1, idx; };                         // idx < 0: none
+__device__ __forceinline__ bool tk_better(const TrackBest &a, const TrackBest &b) {   // a before b in the definition's order
+	if (a.idx < 0) return false;
+	if (b.idx < 0) return true;
+	const unsigned long long l = (unsigned long long) a.d * b.c, r = (unsigned long long) b.d * a.c;
+	return l != r ? l < r : a.l1 != b.l1 ? a.l1 < b.l1 : a.idx < b.idx;
+}
+__global__ void __launch_bounds__(ST_THREADS) st_track_search(const float *__restrict__ F, const float *__restrict__ A, unsigned n,
+                                                              int W, int H, int tx, const StackOffsets *__restrict__ off,
+                                                              const StackTile *__restrict__ tiles, StackTrack *__restrict__ track) {
+	__shared__ __align__(4) unsigned char s_q[ST_TILE_PX * ST_TILE_PX], s_m[ST_TILE_PX * ST_TILE_PX];
+	__shared__ __align__(4) unsigned char s_win[TK_WIN_ROWS * TK_WIN_WORDS * 4];
+	__shared__ TrackBest s_best[ST_THREADS / 32];
+	const int t = blockIdx.x;
+	if (tiles[t].flag != 2) return;
+	const StackWarp cw = st_warp(off, n);
+	const int X0 = (t % tx) * ST_TILE_PX, Y0 = (t / tx) * ST_TILE_PX;
+	{
+		const int X = X0 + (int) (threadIdx.x % ST_TILE_PX), Y = Y0 + (int) (threadIdx.x / ST_TILE_PX);
+		unsigned char qv = 0, mv = 0;
+		float x;
+		if (X < W && Y < H && st_tap(F, cw, (unsigned) Y * (unsigned) W + (unsigned) X, n, &x)) { qv = (unsigned char) st_q(x); mv = 0xff; }
+		s_q[threadIdx.x] = qv; s_m[threadIdx.x] = mv;
+	}
+	for (int e = threadIdx.x; e < TK_WIN_ROWS * TK_WIN_WORDS * 4; e += ST_THREADS) {
+		const int r = e / (TK_WIN_WORDS * 4), b = e - r * (TK_WIN_WORDS * 4);
+		const int X = X0 - TK_LX + b, Y = Y0 - TK_LY + r;
+		s_win[e] = (b < ST_TILE_PX + 2 * TK_LX && X >= 0 && X < W && Y >= 0 && Y < H)
+		           ? (unsigned char) st_q(A[(unsigned) Y * (unsigned) W + (unsigned) X]) : 0;
+	}
+	const int c0 = __syncthreads_count(s_m[threadIdx.x] != 0);
+	const unsigned *q4 = reinterpret_cast<const unsigned *>(s_q), *m4 = reinterpret_cast<const unsigned *>(s_m);
+	const unsigned *w4 = reinterpret_cast<const unsigned *>(s_win);
+	TrackBest best = {0u, 0u, 0, -1};
+	for (int idx = threadIdx.x; idx < TK_NCAND; idx += ST_THREADS) {
+		const int vy = idx / TK_NX - TK_LY, vx = idx % TK_NX - TK_LX;
+		if (vx == 0 && vy == 0) continue;
+		// the tile's rows y and columns x whose source Y0 + y - vy, X0 + x - vx lies inside the raster
+		const int ylo = max(0, vy - Y0), yhi = min(ST_TILE_PX, H - Y0 + vy);
+		const int xlo = max(0, vx - X0), xhi = min(ST_TILE_PX, W - X0 + vx);
+		if (ylo >= yhi || xlo >= xhi) continue;
+		const unsigned cols = (0xffffu >> (ST_TILE_PX - xhi)) & (0xffffu << xlo);
+		unsigned cm[ST_TILE_PX / 4];
+#pragma unroll
+		for (int j = 0; j < ST_TILE_PX / 4; j++) {
+			const unsigned b = cols >> (4 * j);
+			cm[j] = (b & 1u ? 0xffu : 0u) | (b & 2u ? 0xff00u : 0u) | (b & 4u ? 0xff0000u : 0u) | (b & 8u ? 0xff000000u : 0u);
+		}
+		const int sh = TK_LX - vx;                                       // byte of the window row under the tile's column 0
+		const unsigned sel = 0x3210u + 0x1111u * (unsigned) (sh & 3);
+		unsigned D = 0, Cb = 0;
+		for (int y = ylo; y < yhi; y++) {
+			const unsigned *wr = w4 + (y - vy + TK_LY) * TK_WIN_WORDS + (sh >> 2);
+#pragma unroll
+			for (int j = 0; j < ST_TILE_PX / 4; j++) {
+				const unsigned m = m4[y * (ST_TILE_PX / 4) + j] & cm[j];
+				const unsigned d = __vabsdiffu4(q4[y * (ST_TILE_PX / 4) + j], __byte_perm(wr[j], wr[j + 1], sel)) & m;
+				D = __dp4a(d, d, D);
+				Cb += __popc(m);
+			}
+		}
+		const unsigned C = Cb >> 3;
+		if (C == 0 || 2 * C < (unsigned) c0) continue;
+		const TrackBest cand = {D, C, abs(vx) + abs(vy), idx};
+		if (tk_better(cand, best)) best = cand;
+	}
+	for (int o = 16; o > 0; o >>= 1) {
+		TrackBest b;
+		b.d = __shfl_xor_sync(0xffffffffu, best.d, o); b.c = __shfl_xor_sync(0xffffffffu, best.c, o);
+		b.l1 = __shfl_xor_sync(0xffffffffu, best.l1, o); b.idx = __shfl_xor_sync(0xffffffffu, best.idx, o);
+		if (tk_better(b, best)) best = b;
+	}
+	if ((threadIdx.x & 31) == 0) s_best[threadIdx.x >> 5] = best;
+	__syncthreads();
+	if (threadIdx.x == 0) {
+		for (int k = 1; k < ST_THREADS / 32; k++) if (tk_better(s_best[k], best)) best = s_best[k];
+		StackTrack r = {0, 0, 0u, 0u, 0, 0, 0, 0};
+		if (best.idx >= 0) {
+			const unsigned long long e = tiles[t].e, D = best.d, C = best.c;
+			r.vx = best.idx % TK_NX - TK_LX; r.vy = best.idx / TK_NX - TK_LY; r.d = best.d; r.c = best.c;
+			r.moved = !(16ull * D > TSDRGPU_STACK_ADAPT_RATIO * e * C && D > TSDRGPU_STACK_ADAPT_FLOOR * C);
+		}
+		track[t].vx = r.vx; track[t].vy = r.vy; track[t].d = r.d; track[t].c = r.c; track[t].moved = r.moved;
+	}
+}
+
+// track, steps 6b-c: one thread per tile, as st_decide.  Restarts spread from tiles that changed and did not move; the move and
+// the restart the blend takes; the record counts the restarts.
+__global__ void __launch_bounds__(ST_THREADS) st_track_decide(StackTile *__restrict__ tiles, StackTrack *__restrict__ track, int tx,
+                                                              int ty, tsdrgpu_stack_record_t *rec) {
+	const int t = blockIdx.x * blockDim.x + threadIdx.x;
+	bool restart = false;
+	if (t < tx * ty) {
+		const int X = t % tx, Y = t / tx;
+		for (int y = max(Y - 1, 0); y <= min(Y + 1, ty - 1); y++)
+			for (int x = max(X - 1, 0); x <= min(X + 1, tx - 1); x++) restart |= tiles[y * tx + x].flag == 2 && !track[y * tx + x].moved;
+	}
+	if (t < tx * ty) {                                       // flag and moved are only read here, e, bx, by, restart only written
+		StackTile &s = tiles[t];
+		StackTrack &k = track[t];
+		unsigned e = s.e;
+		int bx = 0, by = 0;
+		if (restart) e = ST_NO_LEVEL;
+		else if (s.flag == 2) {                              // changed and not restarting: it moved
+			e = (unsigned) ((7ull * e + 16ull * k.d / k.c) / 8);
+			bx = k.vx; by = k.vy;
+		} else if (s.flag) e = e == ST_NO_LEVEL ? s.r : (unsigned) ((7ull * e + s.r) / 8);
+		s.e = e; k.bx = bx; k.by = by; k.restart = restart;
+	}
+	const unsigned cnt = __reduce_add_sync(0xffffffffu, restart ? 1u : 0u);
+	if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&rec->changed, (int) cnt);
+}
+
+// track, steps 6d and 7: A' and c' at q from A and c at q's source, then out[q + R(o)] from A'[q]
+__global__ void __launch_bounds__(ST_THREADS) st_track_blend(const float *__restrict__ F, const float *__restrict__ A,
+                                                             float *__restrict__ A2, const uint16_t *__restrict__ cnt,
+                                                             uint16_t *__restrict__ cnt2, float *__restrict__ out, unsigned n,
+                                                             int W, int H, int tx, int depth, const StackTrack *__restrict__ track,
+                                                             const StackOffsets *__restrict__ off) {
+	const StackWarp c = st_warp(off, n);
+	for (unsigned q = blockIdx.x * blockDim.x + threadIdx.x; q < n; q += gridDim.x * blockDim.x) {
+		const int Y = (int) (q / (unsigned) W), X = (int) (q - (unsigned) Y * (unsigned) W);
+		const StackTrack &T = track[(Y / ST_TILE_PX) * tx + X / ST_TILE_PX];
+		unsigned s = q;
+		int cs = 0;
+		if (!T.restart) {
+			const int sx = X - T.bx, sy = Y - T.by;
+			if (sx >= 0 && sx < W && sy >= 0 && sy < H) { s = (unsigned) sy * (unsigned) W + (unsigned) sx; cs = cnt[s]; }
+		}
+		const int k = min(cs + 1, depth);
+		float acc = A[s], x;
+		if (st_tap(F, c, q, n, &x)) {
+			const float wn = (float) (1.0 / (double) k), wo = (float) (1.0 - 1.0 / (double) k);
+			acc = __fadd_rn(__fmul_rn(acc, wo), __fmul_rn(x, wn));
+		}
+		A2[q] = acc;
+		cnt2[q] = (uint16_t) k;
+		const unsigned p = st_wrapu(q + c.ro, n);
+		const float fp = __ldg(F + p);
+		out[p] = px_valid(fp) ? acc : fp;
+	}
+}
+
+// track, a restart frame: every c = 1 and no tile moved
+__global__ void __launch_bounds__(ST_THREADS) st_track_init(uint16_t *cnt, unsigned n, StackTrack *track, int ntiles) {
+	for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) cnt[p] = 1;
+	for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < ntiles; t += gridDim.x * blockDim.x) {
+		track[t].bx = 0; track[t].by = 0; track[t].restart = 0;
+	}
+}
+
+template <class T> void st_swap(DeviceBuf<T> &a, DeviceBuf<T> &b) { std::swap(a.ptr, b.ptr); std::swap(a.cap, b.cap); }
+
 }  // namespace
 
-// the accumulator (restarted when the geometry changes), the offsets, the scores and nframes records; nothing may be in flight
+// the accumulator (restarted when the geometry changes), the offsets, the scores and nframes records; in adapt and track modes
+// the tiles, in track mode the second accumulator, the count planes and the search results; nothing may be in flight
 int stack_reserve(tsdrgpu_ctx_t *ctx, StackState *st, int nframes, int w, int h) {
 	if (st->mode == TSDRGPU_STACK_OFF) return TSDRGPU_OK;
 	const size_t n = (size_t) w * h;
-	const size_t ntiles = st->mode == TSDRGPU_STACK_ADAPT ? st_tiles_x(w) * st_tiles_y(h) : 0;
+	const bool track = st->mode == TSDRGPU_STACK_TRACK;
+	const size_t ntiles = st->mode == TSDRGPU_STACK_ADAPT || track ? st_tiles_x(w) * st_tiles_y(h) : 0;
+	const size_t n2 = track ? n : 0, ntrack = track ? ntiles : 0;
 	if (w != st->w || h != st->h) { st->w = w; st->h = h; st->m = 0; }
-	const bool grow = st->d_acc.cap < n || !st->d_off.ptr || st->d_rec.cap < (size_t) nframes || st->d_tiles.cap < ntiles;
+	const bool grow = st->d_acc.cap < n || !st->d_off.ptr || st->d_rec.cap < (size_t) nframes || st->d_tiles.cap < ntiles ||
+	                  st->d_acc2.cap < n2 || st->d_cnt.cap < n2 || st->d_cnt2.cap < n2 || st->d_track.cap < ntrack;
 	if (grow) CU_TRY(ctx, cudaDeviceSynchronize());
 	if (st->d_acc.cap < n) CU_TRY(ctx, st->d_acc.assign(n));
 	if (st->d_tiles.cap < ntiles) CU_TRY(ctx, st->d_tiles.assign(ntiles));
+	if (st->d_acc2.cap < n2) CU_TRY(ctx, st->d_acc2.assign(n2));
+	if (st->d_cnt.cap < n2) CU_TRY(ctx, st->d_cnt.assign(n2));
+	if (st->d_cnt2.cap < n2) CU_TRY(ctx, st->d_cnt2.assign(n2));
+	if (st->d_track.cap < ntrack) CU_TRY(ctx, st->d_track.assign(ntrack));
 	if (st->d_rec.cap < (size_t) nframes) CU_TRY(ctx, st->d_rec.assign(nframes));
 	if (!st->d_off.ptr) {
 		CU_TRY(ctx, st->d_off.assign(2));
@@ -314,7 +491,7 @@ int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const flo
 	const unsigned tiles = (n + ST_TILE - 1) / ST_TILE;
 	unsigned grid = (n + ST_THREADS - 1) / ST_THREADS;
 	if (grid > (unsigned) ctx->sm_count * 8) grid = (unsigned) ctx->sm_count * 8;
-	const bool adapt = st->mode == TSDRGPU_STACK_ADAPT;
+	const bool adapt = st->mode == TSDRGPU_STACK_ADAPT, track = st->mode == TSDRGPU_STACK_TRACK;
 	const int tx = (int) st_tiles_x(w), ty = (int) st_tiles_y(h), ntiles = tx * ty;
 	const unsigned tgrid = (unsigned) (ntiles + ST_THREADS - 1) / ST_THREADS;
 	for (int f = 0; f < nframes; f++) {
@@ -323,14 +500,24 @@ int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const flo
 		tsdrgpu_stack_record_t *rec = st->d_rec.ptr + f;
 		if (st->m == 0) {
 			KL(ctx, "st_restart", stream, st_restart<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, O, n, off, rec));
-			if (adapt) KL(ctx, "st_tile_init", stream, st_tile_init<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, ntiles));
+			if (adapt || track) KL(ctx, "st_tile_init", stream, st_tile_init<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, ntiles));
+			if (track) KL(ctx, "st_track_init", stream, st_track_init<<<grid, ST_THREADS, 0, stream>>>(st->d_cnt.ptr, n, st->d_track.ptr, ntiles));
 		} else {
 			const int m2 = st->m >= 2;
 			const long long k = st->m + 1 < st->depth ? st->m + 1 : st->depth;
 			const float wn = (float) (1.0 / (double) k), wo = (float) (1.0 - 1.0 / (double) k);
 			KL(ctx, "st_score", stream, st_score<<<tiles, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, n, w, st->rx, st->ry, m2, off, st->d_scores.ptr));
 			KL(ctx, "st_pick", stream, st_pick<<<1, 1024, 0, stream>>>(st->d_scores.ptr, w, st->rx, st->ry, m2, off, rec));
-			if (adapt) {
+			if (track) {
+				KL(ctx, "st_tile_sums", stream, st_tile_sums<<<ntiles, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, n, w, h, tx, off, st->d_tiles.ptr));
+				KL(ctx, "st_track_search", stream, st_track_search<<<ntiles, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, n, w, h, tx, off,
+				                                                                                   st->d_tiles.ptr, st->d_track.ptr));
+				KL(ctx, "st_track_decide", stream, st_track_decide<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, st->d_track.ptr, tx, ty, rec));
+				KL(ctx, "st_track_blend", stream, st_track_blend<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, st->d_acc2.ptr, st->d_cnt.ptr,
+				                                                                                st->d_cnt2.ptr, O, n, w, h, tx, st->depth, st->d_track.ptr, off));
+				st_swap(st->d_acc, st->d_acc2);                  // host-side: the next launches on this stream read the new planes
+				st_swap(st->d_cnt, st->d_cnt2);
+			} else if (adapt) {
 				KL(ctx, "st_tile_sums", stream, st_tile_sums<<<ntiles, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, n, w, h, tx, off, st->d_tiles.ptr));
 				KL(ctx, "st_decide", stream, st_decide<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, tx, ty, st->depth, rec));
 				KL(ctx, "st_blend_tiles", stream, st_blend_tiles<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, O, n, (unsigned) w, tx, st->d_tiles.ptr, off));
@@ -382,6 +569,19 @@ int tsdrgpu_stack_set(tsdrgpu_stack_t *s, int mode, int depth, int rx, int ry) {
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, s != NULL);
 	ARG_TRY(s->ctx, stack_ok(mode, depth, rx, ry));
 	return stack_set(&s->st, mode, depth, rx, ry);
+}
+
+int tsdrgpu_stack_vectors(tsdrgpu_stack_t *s, int32_t *h_v, int ntiles) {
+	ARG_TRY((tsdrgpu_ctx_t *) NULL, s != NULL);
+	tsdrgpu_ctx_t *ctx = s->ctx;
+	BIND(ctx);
+	const StackState &st = s->st;
+	ARG_TRY(ctx, h_v && st.mode == TSDRGPU_STACK_TRACK && st.m > 0 && st.d_track.ptr);
+	ARG_TRY(ctx, (size_t) ntiles == st_tiles_x(st.w) * st_tiles_y(st.h));
+	CU_TRY(ctx, cudaDeviceSynchronize());
+	CU_TRY(ctx, cudaMemcpy2D(h_v, 2 * sizeof(int32_t), &st.d_track.ptr[0].bx, sizeof(StackTrack), 2 * sizeof(int32_t), (size_t) ntiles,
+	                         cudaMemcpyDeviceToHost));
+	return TSDRGPU_OK;
 }
 
 int tsdrgpu_stack_run(tsdrgpu_stack_t *s, void *stream_, const float *d_in, float *d_out, int w, int h, int nframes,
