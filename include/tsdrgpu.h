@@ -360,6 +360,9 @@ enum { TSDRGPU_RS_BOX = 0, TSDRGPU_RS_SINC = 1 };
 TSDRGPU_API int  tsdrgpu_resampler_set_kernel(tsdrgpu_resampler_t *r, int kernel);
 /* host-only: the tap table for ratio r in [j][t] order (L*T floats; taps may be NULL to query *T and *L only) */
 TSDRGPU_API int  tsdrgpu_sinc_taps(double r, float *taps, int *T, int *L);
+/* host-only: the pixels per CTA tile a sinc run at ratio r launches with (0 for r < TSDRGPU_SINC_MIN_RATIO); the tests
+ * restate the kernel's tiling and check its shared-memory and history bounds with it */
+TSDRGPU_API uint32_t tsdrgpu_sinc_tile_pixels(double r);
 
 /* ---------------------------------------------------------------------------- a7-a15  frame stage
  * replaces dsp_post_process + dsp_postprocess_t (dsp.c:112-239), dsp_autogain_run (:41-94),

@@ -202,6 +202,7 @@ _SIGS = {
     "tsdrgpu_resampler_set_mag_out": (C.c_int, [C.c_void_p, C.c_void_p]),
     "tsdrgpu_resampler_set_kernel": (C.c_int, [C.c_void_p, C.c_int]),
     "tsdrgpu_sinc_taps": (C.c_int, [C.c_double, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "tsdrgpu_sinc_tile_pixels": (C.c_uint32, [C.c_double]),
     "tsdrgpu_channel_parse": (C.c_int, [C.c_char_p, C.POINTER(ChannelSpec)]),
     "tsdrgpu_channel_taps": (C.c_int, [C.POINTER(ChannelSpec), C.c_uint32, C.c_void_p, C.POINTER(C.c_int)]),
     "tsdrgpu_chanfilt_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),

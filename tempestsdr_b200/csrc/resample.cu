@@ -601,6 +601,10 @@ static int create_handles(tsdrgpu_resampler *r) {
 	return TSDRGPU_OK;
 }
 
+uint32_t tsdrgpu_sinc_tile_pixels(double r) {
+	return r >= TSDRGPU_SINC_MIN_RATIO ? sinc_pixels_per_tile(r) : 0;
+}
+
 int tsdrgpu_resampler_create(tsdrgpu_ctx_t *ctx, tsdrgpu_resampler_t **out) {
 	BIND(ctx); ARG_TRY(ctx, out != NULL);
 	tsdrgpu_resampler *r = new tsdrgpu_resampler();      // value-initialised: every field not set here starts at zero
