@@ -654,8 +654,34 @@ TSDRGPU_API int  tsdrgpu_deblur(tsdrgpu_ctx_t *ctx, void *stream, const float *d
  * The record's `changed` counts the tiles restarted in the frame, as in adapt; tsdrgpu_stack_vectors reads where each tile
  * moved.  LX and LY are fixed: 32 lines cover a one-line scroll of any usual font.  When no tile moves in a sequence, a tile's
  * pixels share one count equal to adapt's m_t, so every output and record equals adapt's bit for bit. */
+/* The glitch-tolerant mode (TSDRGPU_STACK_ROBUST, "robust:<N>[:<rx>x<ry>]", the same ranges and defaults) is track with three
+ * additions that keep a disturbance lasting one frame out of the average: a frame torn around dropped samples, a re-centring step
+ * or a PLL correction that moves one frame against the next, impulsive interference over a few lines.  In adapt and track every
+ * tile such a frame touches restarts with that one noisy frame as its content, and the average takes N frames to rebuild.  Here
+ * a change must last two frames before a tile restarts.  Steps 1-5 and 7, 6a, 6t, the move test, and 6c for tiles that blend are
+ * track's, unchanged, and so are the per-pixel counts, except that bit 15 of c[p] holds a flag g[p] and the count is c[p] & 0x7fff
+ * (still <= N).  Per tile one more bit, pend_t; a restart frame, and so every restart of align, sets every pend_t = 0 and g = 0.
+ *   6r. debounce: new_t = changed_t && !moved_t (the tile's own flag of track's 6b), confirmed_t = new_t && pend_t.  A tile
+ *      restarts when confirmed_t holds for it or one of its 8 neighbours (no wrap); a moved tile that a neighbour restarts does
+ *      restart.  A tile is held when new_t && !pend_t and no neighbour restarts it.
+ *   6h. frame hold: with `held` the number of held tiles, the frame is a glitch frame when 2 held > ntiles.  Then o = b (step 3's
+ *      prediction) replaces the found offset in step 7 and in the history (o2 = o1, o1 = b); no tile blends, moves or restarts;
+ *      A, c and every e_t stay as they were.  The record reports offset = b, score, dx and dy as found, and changed = 0.
+ *   6c. a held tile keeps e_t; a restarting tile takes e_t = none; every other tile follows track's 6c.
+ *   6d. a held tile keeps A and c (g included).  Every other tile blends as in track with k = min((c[s] & 0x7fff) + 1, N), except
+ *      that the gate applies in a tile that neither restarts nor is held and whose level before this frame's 6c is e_t != none:
+ *      for a pixel p whose four taps are valid and whose source s lies inside the raster, d = Q(x[p]) - Q(A[s]), and p is gated
+ *      when d^2 > max(e_t, GATE_MIN) (more than 4 rms of the tile's residual and more than 32 levels; GATE_MIN =
+ *      TSDRGPU_STACK_ROBUST_GATE_MIN = 16 FLOOR).  A gated p with g[s] = 0 keeps A'[p] = A[s] and c'[p] = (c[s] & 0x7fff) | 0x8000;
+ *      a gated p with g[s] = 1 restarts, A'[p] = x[p] and c'[p] = 1.  Every pixel not gated takes track's 6d with g cleared.
+ *   After every frame, glitch frames included, pend_t = new_t for every tile.
+ * A region that keeps changing restarts every third frame (restart, fresh level, held, restart), where adapt and track restart
+ * it every second frame: the frame after a restart measures against e_t = none, so it is never new.  A lasting change is taken
+ * one frame later than in track, and a lone bad frame never reaches the average.  The constants are fixed.  When no tile is
+ * held and no pixel gated over a sequence, no tile is ever new (the first would have been held), so every output and record
+ * equals track's bit for bit.  tsdrgpu_stack_robust_counts reads the last frame's held tiles, gated pixels and hold. */
 /* the stack's modes; any other value, 2, 3 and 5 included, is refused with TSDRGPU_EINVAL */
-enum { TSDRGPU_STACK_OFF = 0, TSDRGPU_STACK_ALIGN = 1, TSDRGPU_STACK_ADAPT = 4, TSDRGPU_STACK_TRACK = 8 };
+enum { TSDRGPU_STACK_OFF = 0, TSDRGPU_STACK_ALIGN = 1, TSDRGPU_STACK_ADAPT = 4, TSDRGPU_STACK_TRACK = 8, TSDRGPU_STACK_ROBUST = 16 };
 #define TSDRGPU_STACK_MIN_N  2
 #define TSDRGPU_STACK_MAX_N  1024
 #define TSDRGPU_STACK_MAX_RX 32
@@ -665,15 +691,16 @@ enum { TSDRGPU_STACK_OFF = 0, TSDRGPU_STACK_ALIGN = 1, TSDRGPU_STACK_ADAPT = 4, 
 #define TSDRGPU_STACK_ADAPT_FLOOR 64
 #define TSDRGPU_STACK_TRACK_LX 16
 #define TSDRGPU_STACK_TRACK_LY 32
+#define TSDRGPU_STACK_ROBUST_GATE_MIN (16 * TSDRGPU_STACK_ADAPT_FLOOR)
 typedef struct {
 	double  offset;                               /* o (unwrapped; 0 on a restart frame) */
 	int64_t score;                                /* S(s*) (0 on a restart frame) */
 	int32_t dx, dy;                               /* the best candidate's place in the window */
 	int32_t restarted;                            /* 1 on a restart frame */
-	int32_t changed;                              /* adapt, track: the tiles restarted in this frame (0 for align) */
+	int32_t changed;                              /* adapt, track, robust: the tiles restarted in this frame (0 for align) */
 } tsdrgpu_stack_record_t;
 /* host-only: the spelling shared by the host library's TSDR_STACK and Python.  "off", "align:<N>", "align:<N>:<rx>x<ry>", and
- * the same with "adapt:" or "track:"; N, rx, ry = one to six digits in the ranges above, rx and ry defaulting to 8 and 2.
+ * the same with "adapt:", "track:" or "robust:"; N, rx, ry = one to six digits in the ranges above, rx and ry defaulting to 8, 2.
  * Nothing else (no sign, blank or point).  TSDRGPU_OK with the four outputs set (zeros for "off"), else TSDRGPU_EINVAL and the
  * outputs untouched. */
 TSDRGPU_API int  tsdrgpu_stack_parse(const char *spec, int *mode, int *depth, int *rx, int *ry);
@@ -687,11 +714,16 @@ TSDRGPU_API int  tsdrgpu_stack_reset(tsdrgpu_stack_t *st);
 TSDRGPU_API int  tsdrgpu_stack_set(tsdrgpu_stack_t *st, int mode, int depth, int rx, int ry);
 TSDRGPU_API int  tsdrgpu_stack_run(tsdrgpu_stack_t *st, void *stream, const float *d_in, float *d_out, int w, int h, int nframes,
                                    tsdrgpu_stack_record_t *h_records_pinned);
-/* track mode (synchronises): where each tile of the last frame moved.  h_v receives 2 ntiles values, (vx, vy) of tile t at
- * h_v[2t], h_v[2t + 1] with t = (Y div 16) ceil(W / 16) + X div 16: v* for a tile that moved and did not restart, (0, 0) (never a
- * candidate) for every other tile and on a restart frame.  TSDRGPU_EINVAL unless the mode is track, a frame has been taken since
- * the last restart and ntiles is the tile count of its geometry. */
+/* track and robust modes (synchronises): where each tile of the last frame moved.  h_v receives 2 ntiles values, (vx, vy) of
+ * tile t at h_v[2t], h_v[2t + 1] with t = (Y div 16) ceil(W / 16) + X div 16: v* for a tile that moved and did not restart (nor,
+ * in robust mode, was held), (0, 0) (never a candidate) for every other tile, on a restart frame and on a glitch frame.
+ * TSDRGPU_EINVAL unless the mode is track or robust, a frame has been taken since the last restart and ntiles is the tile count
+ * of its geometry. */
 TSDRGPU_API int  tsdrgpu_stack_vectors(tsdrgpu_stack_t *st, int32_t *h_v, int ntiles);
+/* robust mode (synchronises): the last frame's held tiles (6r), gated pixels (6d) and whether it was a glitch frame (6h, 0 or
+ * 1); all three 0 on a restart frame.  TSDRGPU_EINVAL unless the mode is robust and a frame has been taken since the last
+ * restart. */
+TSDRGPU_API int  tsdrgpu_stack_robust_counts(tsdrgpu_stack_t *st, int32_t *held_tiles, uint64_t *gated_pixels, int32_t *frame_held);
 /* the frame stage's stack mode, applied from the next run on.  The mode is kept across tsdrgpu_framestage_reset; the accumulator
  * is not (the reset restarts it).  Out-of-range values or an unknown mode: TSDRGPU_EINVAL. */
 TSDRGPU_API int  tsdrgpu_framestage_set_stack(tsdrgpu_framestage_t *fs, int mode, int depth, int rx, int ry);
@@ -918,7 +950,7 @@ TSDRGPU_API int  tsdrgpu_pipeline_set_denoise(tsdrgpu_pipeline_t *p, int mode, i
 /* deblur mode (TSDRGPU_DEBLUR_OFF, the default, or TSDRGPU_DEBLUR_RL; see tsdrgpu_framestage_set_deblur), taking effect at the
  * next frame-stage batch */
 TSDRGPU_API int  tsdrgpu_pipeline_set_deblur(tsdrgpu_pipeline_t *p, int mode, int sigma_centi, int iterations);
-/* stack mode (TSDRGPU_STACK_OFF, the default, TSDRGPU_STACK_ALIGN, TSDRGPU_STACK_ADAPT or TSDRGPU_STACK_TRACK; see tsdrgpu_framestage_set_stack),
+/* stack mode (TSDRGPU_STACK_OFF, the default, TSDRGPU_STACK_ALIGN, TSDRGPU_STACK_ADAPT, TSDRGPU_STACK_TRACK or TSDRGPU_STACK_ROBUST; see tsdrgpu_framestage_set_stack),
  * taking effect at the next frame-stage batch.  tsdrgpu_pipeline_sync restarts the stack at the next frame-stage batch.  While
  * the stack is on, every frame with an auto-gain report (dsp.c:231-235) also announces value id TSDRGPU_VALUE_ID_STACK_DRIFT with arg0 = the mean drift
  * in px/frame since the last announcement or restart ((o - o_last) / frames, 0 right after a restart) and arg1 = the frame's

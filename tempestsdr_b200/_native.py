@@ -144,7 +144,7 @@ def deblur_mode(spec: str):
     return tuple(o.value for o in out)
 
 
-STACK_OFF, STACK_ALIGN, STACK_ADAPT, STACK_TRACK = 0, 1, 4, 8   # TSDRGPU_STACK_OFF / _ALIGN / _ADAPT / _TRACK
+STACK_OFF, STACK_ALIGN, STACK_ADAPT, STACK_TRACK, STACK_ROBUST = 0, 1, 4, 8, 16   # TSDRGPU_STACK_OFF / _ALIGN / _ADAPT / _TRACK / _ROBUST
 VALUE_ID_STACK_DRIFT = 101                          # TSDRGPU_VALUE_ID_STACK_DRIFT
 
 
@@ -155,11 +155,11 @@ class StackRecord(C.Structure):
 
 
 def stack_mode(spec: str):
-    """"off", "align:<N>[:<rx>x<ry>]", "adapt:<N>[:<rx>x<ry>]" or "track:<N>[:<rx>x<ry>]" (the host library's TSDR_STACK
-    spelling) -> (mode, N, rx, ry), read by tsdrgpu_stack_parse."""
+    """"off", "align:<N>[:<rx>x<ry>]", "adapt:<N>[:<rx>x<ry>]", "track:<N>[:<rx>x<ry>]" or "robust:<N>[:<rx>x<ry>]" (the host
+    library's TSDR_STACK spelling) -> (mode, N, rx, ry), read by tsdrgpu_stack_parse."""
     out = [C.c_int() for _ in range(4)]
     if lib().tsdrgpu_stack_parse(spec.encode(), *[C.byref(o) for o in out]) != 0:
-        raise ValueError(f"stack must be 'off', 'align:<N>[:<rx>x<ry>]', 'adapt:<N>[:<rx>x<ry>]' or 'track:<N>[:<rx>x<ry>]' with N in [2, 1024], rx in [1, 32] and ry in [0, 8], not {spec!r}")
+        raise ValueError(f"stack must be 'off', 'align:<N>[:<rx>x<ry>]', 'adapt:<N>[:<rx>x<ry>]', 'track:<N>[:<rx>x<ry>]' or 'robust:<N>[:<rx>x<ry>]' with N in [2, 1024], rx in [1, 32] and ry in [0, 8], not {spec!r}")
     return tuple(o.value for o in out)
 
 
@@ -258,6 +258,7 @@ _SIGS = {
     "tsdrgpu_stack_set": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_stack_run": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "tsdrgpu_stack_vectors": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "tsdrgpu_stack_robust_counts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tsdrgpu_framestage_set_stack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "tsdrgpu_framestage_stack_records": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "tsdrgpu_framestage_join": (C.c_int, [C.c_void_p, C.c_void_p]),

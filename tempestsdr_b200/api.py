@@ -250,8 +250,8 @@ class Stack:
 
     def set(self, spec: str) -> None:
         """"off", "align:<N>[:<rx>x<ry>]", "adapt:<N>[:<rx>x<ry>]" (restarting tile by tile where the picture changes) or
-        "track:<N>[:<rx>x<ry>]" (carrying each tile's average with content that moves) from the next run on; new settings
-        restart the average."""
+        "track:<N>[:<rx>x<ry>]" (carrying each tile's average with content that moves) or "robust:<N>[:<rx>x<ry>]" (track,
+        ignoring disturbances that last one frame) from the next run on; new settings restart the average."""
         self.ctx.chk(self.ctx._lib.tsdrgpu_stack_set(self._h, *N.stack_mode(spec)))
 
     def reset(self) -> None:
@@ -274,12 +274,18 @@ class Stack:
         return out, [N.StackRecord.from_buffer_copy(r) for r in recs]
 
     def vectors(self, width: int, height: int) -> np.ndarray:
-        """Track mode: where each 16 x 16 tile of the last frame moved -> (tiles down, tiles across, 2) int32 of (vx, vy), (0, 0)
+        """Track and robust modes: where each 16 x 16 tile of the last frame moved -> (tiles down, tiles across, 2) int32 of (vx, vy), (0, 0)
         for tiles that did not move or restarted.  Synchronises the device."""
         ty, tx = (height + 15) // 16, (width + 15) // 16
         v = np.zeros((ty, tx, 2), np.int32)
         self.ctx.chk(self.ctx._lib.tsdrgpu_stack_vectors(self._h, v.ctypes.data, ty * tx))
         return v
+
+    def robust_counts(self) -> tuple:
+        """Robust mode: the last frame's (held tiles, gated pixels, glitch frame as a bool).  Synchronises the device."""
+        held, gated, hold = C.c_int32(), C.c_uint64(), C.c_int32()
+        self.ctx.chk(self.ctx._lib.tsdrgpu_stack_robust_counts(self._h, C.byref(held), C.byref(gated), C.byref(hold)))
+        return held.value, gated.value, bool(hold.value)
 
 
 class _SegmentReports:
@@ -563,7 +569,9 @@ class PostProcessor:
     def set_stack(self, spec: str) -> None:
         """"off" (the default), "align:<N>[:<rx>x<ry>]" (drift-registered averaging of the delivered frames, ahead of NLM and
         CLAHE, tsdrgpu.h), "adapt:<N>[:<rx>x<ry>]" (the same, restarting tile by tile where the picture changes) or
-        "track:<N>[:<rx>x<ry>]" (the same, carrying each tile's average with content that scrolls or moves) for the following runs; the mode is kept across reset, the average restarts there."""
+        "track:<N>[:<rx>x<ry>]" (the same, carrying each tile's average with content that scrolls or moves) or
+        "robust:<N>[:<rx>x<ry>]" (track, ignoring disturbances that last one frame) for the following runs; the mode is kept
+        across reset, the average restarts there."""
         self.ctx.chk(self.ctx._lib.tsdrgpu_framestage_set_stack(self._h, *N.stack_mode(spec)))
 
     def stack_records(self, nframes: int):

@@ -132,6 +132,17 @@ struct StackTrack {                              // track: one per tile of the a
 	int bx, by;                                  // decide: the move the blend takes, (0, 0) unless moved and not restarting
 	int restart;                                 // decide: the tile restarts
 };
+struct StackRobust {                             // robust: one per tile of the accumulator
+	int pend;                                    // pend_t: the tile was new in the last frame
+	int confirmed;                               // decide: confirmed_t of this frame
+	int held;                                    // decide: the tile is held this frame
+	unsigned gate_e;                             // decide: e_t before this frame's 6c where the gate applies, else 0xffffffff
+};
+struct StackRobustFrame {                        // robust: the frame in flight
+	double b;                                    // step 3's prediction b of the next frame
+	int held, hold;                              // held tiles, and 1 on a glitch frame
+	unsigned long long gated;                    // gated pixels
+};
 struct StackState {
 	int mode, depth, rx, ry;                     // TSDRGPU_STACK_* and its parameters (N, rx, ry)
 	int w, h;                                    // the accumulator's geometry
@@ -141,10 +152,12 @@ struct StackState {
 	DeviceBuf<double> d_off;                     // o1, o2
 	DeviceBuf<unsigned long long> d_scores;      // S of every candidate of the frame in flight
 	DeviceBuf<tsdrgpu_stack_record_t> d_rec;     // the records of a batch
-	DeviceBuf<StackTile> d_tiles;                // adapt, track: one per tile of the accumulator
-	DeviceBuf<float> d_acc2;                     // track: A', swapped with d_acc after every frame
-	DeviceBuf<uint16_t> d_cnt, d_cnt2;           // track: c and c', swapped likewise
-	DeviceBuf<StackTrack> d_track;               // track: one per tile of the accumulator
+	DeviceBuf<StackTile> d_tiles;                // adapt, track, robust: one per tile of the accumulator
+	DeviceBuf<float> d_acc2;                     // track, robust: A', swapped with d_acc after every frame
+	DeviceBuf<uint16_t> d_cnt, d_cnt2;           // track, robust: c and c', swapped likewise
+	DeviceBuf<StackTrack> d_track;               // track, robust: one per tile of the accumulator
+	DeviceBuf<StackRobust> d_robust;             // robust: one per tile of the accumulator
+	DeviceBuf<StackRobustFrame> d_rframe;        // robust: one
 };
 int stack_reserve(tsdrgpu_ctx_t *ctx, StackState *st, int nframes, int w, int h);
 int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const float *in, float *out, int nframes, int w, int h);

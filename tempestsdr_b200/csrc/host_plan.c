@@ -248,7 +248,8 @@ int denoise_ok(int mode, int h_milli, int r, int p) {
 }
 
 int stack_ok(int mode, int depth, int rx, int ry) {
-	return mode == TSDRGPU_STACK_OFF || ((mode == TSDRGPU_STACK_ALIGN || mode == TSDRGPU_STACK_ADAPT || mode == TSDRGPU_STACK_TRACK) && depth >= TSDRGPU_STACK_MIN_N &&
+	return mode == TSDRGPU_STACK_OFF || ((mode == TSDRGPU_STACK_ALIGN || mode == TSDRGPU_STACK_ADAPT || mode == TSDRGPU_STACK_TRACK ||
+	                                      mode == TSDRGPU_STACK_ROBUST) && depth >= TSDRGPU_STACK_MIN_N &&
 	       depth <= TSDRGPU_STACK_MAX_N && rx >= 1 && rx <= TSDRGPU_STACK_MAX_RX && ry >= 0 && ry <= TSDRGPU_STACK_MAX_RY);
 }
 
@@ -314,6 +315,7 @@ int tsdrgpu_stack_parse(const char *spec, int *mode, int *depth, int *rx, int *r
 	if (!spec || !mode || !depth || !rx || !ry) return TSDRGPU_EINVAL;
 	if ((on = option_parse(spec, "align:", 0, 'x', 8, 2, v)) < 0) { on = option_parse(spec, "adapt:", 0, 'x', 8, 2, v); m = TSDRGPU_STACK_ADAPT; }
 	if (on < 0) { on = option_parse(spec, "track:", 0, 'x', 8, 2, v); m = TSDRGPU_STACK_TRACK; }
+	if (on < 0) { on = option_parse(spec, "robust:", 0, 'x', 8, 2, v); m = TSDRGPU_STACK_ROBUST; }
 	if (on < 0) return TSDRGPU_EINVAL;
 	if (!on) m = TSDRGPU_STACK_OFF;
 	if (!stack_ok(m, v[0], v[1], v[2])) return TSDRGPU_EINVAL;

@@ -6,7 +6,9 @@
 // st_blend_tiles blends with those.  The tracking mode keeps st_tile_sums and replaces the other two: st_track_search looks for
 // where each changed tile's content came from, st_track_decide restarts the tiles that changed and did not move (and their
 // neighbours), and st_track_blend gathers the accumulator and the per-pixel counts along each tile's move into the second
-// planes, which the host swaps with the first after every frame.  No host round trip inside a batch, and no CTA waits for another.  Built with -fmad=false;
+// planes, which the host swaps with the first after every frame.  The glitch-tolerant mode keeps the tracking mode's first two
+// and replaces the other two: st_robust_decide (one CTA) adds the debounce, counts the held tiles and decides a glitch frame, and
+// st_robust_blend adds the pixel gate.  No host round trip inside a batch, and no CTA waits for another.  Built with -fmad=false;
 // the float arithmetic is spelled with __f*_rn anyway, so every output bit follows the definition.
 #include "common.cuh"
 #include "host_plan.h"
@@ -452,21 +454,144 @@ __global__ void __launch_bounds__(ST_THREADS) st_track_init(uint16_t *cnt, unsig
 	}
 }
 
+// robust, steps 6r, 6h and 6c: one CTA for the whole tile grid, so that the held count and the glitch-frame decision need no
+// second launch.  Pass 1 marks the confirmed tiles, pass 2 spreads their restarts and counts the held tiles, pass 3 sets each
+// tile's level, move, restart, gate level and pend for the blend.  Thread 0 then keeps a glitch frame's prediction as the
+// offset (st_warp in st_robust_blend reads it for the output) and the record's, and leaves the next frame's prediction.
+constexpr int RB_THREADS = 1024;
+constexpr uint16_t RB_GATED = 0x8000u, RB_COUNT = 0x7fffu;
+__global__ void __launch_bounds__(RB_THREADS) st_robust_decide(StackTile *__restrict__ tiles, StackTrack *__restrict__ track,
+                                                               StackRobust *__restrict__ rob, int tx, int ty, StackOffsets *off,
+                                                               StackRobustFrame *fr, tsdrgpu_stack_record_t *rec) {
+	__shared__ int s_held, s_restarts;
+	const int ntiles = tx * ty;
+	if (threadIdx.x == 0) { s_held = 0; s_restarts = 0; }
+	for (int t = threadIdx.x; t < ntiles; t += RB_THREADS)
+		rob[t].confirmed = tiles[t].flag == 2 && !track[t].moved && rob[t].pend;
+	__syncthreads();
+	int held = 0;
+	for (int t = threadIdx.x; t < ntiles; t += RB_THREADS) {
+		const int X = t % tx, Y = t / tx;
+		bool restart = false;
+		for (int y = max(Y - 1, 0); y <= min(Y + 1, ty - 1); y++)
+			for (int x = max(X - 1, 0); x <= min(X + 1, tx - 1); x++) restart |= rob[y * tx + x].confirmed != 0;
+		const bool h = tiles[t].flag == 2 && !track[t].moved && !rob[t].pend && !restart;
+		track[t].restart = restart;
+		rob[t].held = h;
+		held += h;
+	}
+	held = (int) __reduce_add_sync(0xffffffffu, (unsigned) held);
+	if ((threadIdx.x & 31) == 0 && held) atomicAdd(&s_held, held);
+	__syncthreads();
+	const bool hold = 2 * s_held > ntiles;
+	int restarts = 0;
+	for (int t = threadIdx.x; t < ntiles; t += RB_THREADS) {   // every read and write here is of tile t's own entries
+		StackTile &s = tiles[t];
+		StackTrack &k = track[t];
+		StackRobust &r = rob[t];
+		unsigned e = s.e, ge = ST_NO_LEVEL;
+		int bx = 0, by = 0;
+		bool restart = k.restart && !hold;
+		if (restart) e = ST_NO_LEVEL;
+		else if (!hold && !r.held) {
+			ge = e;
+			if (s.flag == 2) {                                 // changed, not restarting, not held: it moved
+				e = (unsigned) ((7ull * e + 16ull * k.d / k.c) / 8);
+				bx = k.vx; by = k.vy;
+			} else if (s.flag) e = e == ST_NO_LEVEL ? s.r : (unsigned) ((7ull * e + s.r) / 8);
+		}
+		s.e = e; k.bx = bx; k.by = by; k.restart = restart;
+		r.gate_e = ge; r.pend = s.flag == 2 && !k.moved;
+		restarts += restart;
+	}
+	restarts = (int) __reduce_add_sync(0xffffffffu, (unsigned) restarts);
+	if ((threadIdx.x & 31) == 0 && restarts) atomicAdd(&s_restarts, restarts);
+	__syncthreads();
+	if (threadIdx.x == 0) {
+		if (hold) { off->o1 = fr->b; rec->offset = fr->b; }
+		rec->changed = s_restarts;
+		fr->held = s_held; fr->hold = hold; fr->gated = 0;
+		fr->b = st_base(off, 1);                              // every later frame has m >= 2
+	}
+}
+
+// robust, steps 6d and 7: track's gather and blend with the pixel gate; held tiles and a glitch frame copy A and c over
+__global__ void __launch_bounds__(ST_THREADS) st_robust_blend(const float *__restrict__ F, const float *__restrict__ A,
+                                                              float *__restrict__ A2, const uint16_t *__restrict__ cnt,
+                                                              uint16_t *__restrict__ cnt2, float *__restrict__ out, unsigned n,
+                                                              int W, int H, int tx, int depth, const StackTrack *__restrict__ track,
+                                                              const StackRobust *__restrict__ rob,
+                                                              StackRobustFrame *fr, const StackOffsets *__restrict__ off) {
+	const StackWarp c = st_warp(off, n);                      // on a glitch frame o1 = b already: the output moves by R(b)
+	const bool hold = fr->hold;
+	unsigned gated = 0;
+	for (unsigned q = blockIdx.x * blockDim.x + threadIdx.x; q < n; q += gridDim.x * blockDim.x) {
+		const int Y = (int) (q / (unsigned) W), X = (int) (q - (unsigned) Y * (unsigned) W);
+		const int t = (Y / ST_TILE_PX) * tx + X / ST_TILE_PX;
+		float acc;
+		unsigned c2;
+		if (hold || rob[t].held) { acc = A[q]; c2 = cnt[q]; }
+		else {
+			const StackTrack &T = track[t];
+			unsigned s = q, cs = 0, g = 0;
+			bool inside = false;
+			if (!T.restart) {
+				const int sx = X - T.bx, sy = Y - T.by;
+				if (sx >= 0 && sx < W && sy >= 0 && sy < H) {
+					s = (unsigned) sy * (unsigned) W + (unsigned) sx;
+					cs = cnt[s]; g = cs & RB_GATED; cs &= RB_COUNT; inside = true;
+				}
+			}
+			const int k = min((int) cs + 1, depth);
+			acc = A[s]; c2 = (unsigned) k;
+			float x;
+			if (st_tap(F, c, q, n, &x)) {
+				const unsigned ge = rob[t].gate_e;
+				const int d = (int) st_q(x) - (int) st_q(acc);
+				if (inside && ge != ST_NO_LEVEL && (unsigned) (d * d) > max(ge, (unsigned) TSDRGPU_STACK_ROBUST_GATE_MIN)) {
+					gated++;
+					if (g) { acc = x; c2 = 1; }
+					else c2 = cs | RB_GATED;
+				} else {
+					const float wn = (float) (1.0 / (double) k), wo = (float) (1.0 - 1.0 / (double) k);
+					acc = __fadd_rn(__fmul_rn(acc, wo), __fmul_rn(x, wn));
+				}
+			}
+		}
+		A2[q] = acc;
+		cnt2[q] = (uint16_t) c2;
+		const unsigned p = st_wrapu(q + c.ro, n);
+		const float fp = __ldg(F + p);
+		out[p] = px_valid(fp) ? acc : fp;
+	}
+	gated = __reduce_add_sync(0xffffffffu, gated);
+	if ((threadIdx.x & 31) == 0 && gated) atomicAdd(&fr->gated, (unsigned long long) gated);
+}
+
+// robust, a restart frame (after st_track_init): every pend_t = 0, and the next frame's prediction b = R(0) = 0
+__global__ void __launch_bounds__(ST_THREADS) st_robust_init(StackRobust *rob, int ntiles, StackRobustFrame *fr) {
+	const int t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t < ntiles) { rob[t].pend = 0; rob[t].confirmed = 0; rob[t].held = 0; rob[t].gate_e = ST_NO_LEVEL; }
+	if (t == 0) { fr->b = 0.0; fr->held = 0; fr->hold = 0; fr->gated = 0; }
+}
+
 template <class T> void st_swap(DeviceBuf<T> &a, DeviceBuf<T> &b) { std::swap(a.ptr, b.ptr); std::swap(a.cap, b.cap); }
 
 }  // namespace
 
-// the accumulator (restarted when the geometry changes), the offsets, the scores and nframes records; in adapt and track modes
-// the tiles, in track mode the second accumulator, the count planes and the search results; nothing may be in flight
+// the accumulator (restarted when the geometry changes), the offsets, the scores and nframes records; in adapt, track and robust
+// modes the tiles, in track and robust modes the second accumulator, the count planes and the search results, in robust mode
+// the debounce state; nothing may be in flight
 int stack_reserve(tsdrgpu_ctx_t *ctx, StackState *st, int nframes, int w, int h) {
 	if (st->mode == TSDRGPU_STACK_OFF) return TSDRGPU_OK;
 	const size_t n = (size_t) w * h;
-	const bool track = st->mode == TSDRGPU_STACK_TRACK;
+	const bool robust = st->mode == TSDRGPU_STACK_ROBUST, track = st->mode == TSDRGPU_STACK_TRACK || robust;
 	const size_t ntiles = st->mode == TSDRGPU_STACK_ADAPT || track ? st_tiles_x(w) * st_tiles_y(h) : 0;
-	const size_t n2 = track ? n : 0, ntrack = track ? ntiles : 0;
+	const size_t n2 = track ? n : 0, ntrack = track ? ntiles : 0, nrobust = robust ? ntiles : 0;
 	if (w != st->w || h != st->h) { st->w = w; st->h = h; st->m = 0; }
 	const bool grow = st->d_acc.cap < n || !st->d_off.ptr || st->d_rec.cap < (size_t) nframes || st->d_tiles.cap < ntiles ||
-	                  st->d_acc2.cap < n2 || st->d_cnt.cap < n2 || st->d_cnt2.cap < n2 || st->d_track.cap < ntrack;
+	                  st->d_acc2.cap < n2 || st->d_cnt.cap < n2 || st->d_cnt2.cap < n2 || st->d_track.cap < ntrack ||
+	                  st->d_robust.cap < nrobust || (robust && !st->d_rframe.ptr);
 	if (grow) CU_TRY(ctx, cudaDeviceSynchronize());
 	if (st->d_acc.cap < n) CU_TRY(ctx, st->d_acc.assign(n));
 	if (st->d_tiles.cap < ntiles) CU_TRY(ctx, st->d_tiles.assign(ntiles));
@@ -474,6 +599,8 @@ int stack_reserve(tsdrgpu_ctx_t *ctx, StackState *st, int nframes, int w, int h)
 	if (st->d_cnt.cap < n2) CU_TRY(ctx, st->d_cnt.assign(n2));
 	if (st->d_cnt2.cap < n2) CU_TRY(ctx, st->d_cnt2.assign(n2));
 	if (st->d_track.cap < ntrack) CU_TRY(ctx, st->d_track.assign(ntrack));
+	if (st->d_robust.cap < nrobust) CU_TRY(ctx, st->d_robust.assign(nrobust));
+	if (robust && !st->d_rframe.ptr) CU_TRY(ctx, st->d_rframe.assign(1));
 	if (st->d_rec.cap < (size_t) nframes) CU_TRY(ctx, st->d_rec.assign(nframes));
 	if (!st->d_off.ptr) {
 		CU_TRY(ctx, st->d_off.assign(2));
@@ -491,7 +618,8 @@ int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const flo
 	const unsigned tiles = (n + ST_TILE - 1) / ST_TILE;
 	unsigned grid = (n + ST_THREADS - 1) / ST_THREADS;
 	if (grid > (unsigned) ctx->sm_count * 8) grid = (unsigned) ctx->sm_count * 8;
-	const bool adapt = st->mode == TSDRGPU_STACK_ADAPT, track = st->mode == TSDRGPU_STACK_TRACK;
+	const bool adapt = st->mode == TSDRGPU_STACK_ADAPT, robust = st->mode == TSDRGPU_STACK_ROBUST;
+	const bool track = st->mode == TSDRGPU_STACK_TRACK || robust;
 	const int tx = (int) st_tiles_x(w), ty = (int) st_tiles_y(h), ntiles = tx * ty;
 	const unsigned tgrid = (unsigned) (ntiles + ST_THREADS - 1) / ST_THREADS;
 	for (int f = 0; f < nframes; f++) {
@@ -502,6 +630,7 @@ int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const flo
 			KL(ctx, "st_restart", stream, st_restart<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, O, n, off, rec));
 			if (adapt || track) KL(ctx, "st_tile_init", stream, st_tile_init<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, ntiles));
 			if (track) KL(ctx, "st_track_init", stream, st_track_init<<<grid, ST_THREADS, 0, stream>>>(st->d_cnt.ptr, n, st->d_track.ptr, ntiles));
+			if (robust) KL(ctx, "st_robust_init", stream, st_robust_init<<<tgrid, ST_THREADS, 0, stream>>>(st->d_robust.ptr, ntiles, st->d_rframe.ptr));
 		} else {
 			const int m2 = st->m >= 2;
 			const long long k = st->m + 1 < st->depth ? st->m + 1 : st->depth;
@@ -512,9 +641,17 @@ int stack_run(tsdrgpu_ctx_t *ctx, StackState *st, cudaStream_t stream, const flo
 				KL(ctx, "st_tile_sums", stream, st_tile_sums<<<ntiles, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, n, w, h, tx, off, st->d_tiles.ptr));
 				KL(ctx, "st_track_search", stream, st_track_search<<<ntiles, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, n, w, h, tx, off,
 				                                                                                   st->d_tiles.ptr, st->d_track.ptr));
-				KL(ctx, "st_track_decide", stream, st_track_decide<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, st->d_track.ptr, tx, ty, rec));
-				KL(ctx, "st_track_blend", stream, st_track_blend<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, st->d_acc2.ptr, st->d_cnt.ptr,
-				                                                                                st->d_cnt2.ptr, O, n, w, h, tx, st->depth, st->d_track.ptr, off));
+				if (robust) {
+					KL(ctx, "st_robust_decide", stream, st_robust_decide<<<1, RB_THREADS, 0, stream>>>(st->d_tiles.ptr, st->d_track.ptr, st->d_robust.ptr,
+					                                                                                 tx, ty, off, st->d_rframe.ptr, rec));
+					KL(ctx, "st_robust_blend", stream, st_robust_blend<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, st->d_acc2.ptr, st->d_cnt.ptr,
+					                                                                                  st->d_cnt2.ptr, O, n, w, h, tx, st->depth, st->d_track.ptr,
+					                                                                                  st->d_robust.ptr, st->d_rframe.ptr, off));
+				} else {
+					KL(ctx, "st_track_decide", stream, st_track_decide<<<tgrid, ST_THREADS, 0, stream>>>(st->d_tiles.ptr, st->d_track.ptr, tx, ty, rec));
+					KL(ctx, "st_track_blend", stream, st_track_blend<<<grid, ST_THREADS, 0, stream>>>(F, st->d_acc.ptr, st->d_acc2.ptr, st->d_cnt.ptr,
+					                                                                                st->d_cnt2.ptr, O, n, w, h, tx, st->depth, st->d_track.ptr, off));
+				}
 				st_swap(st->d_acc, st->d_acc2);                  // host-side: the next launches on this stream read the new planes
 				st_swap(st->d_cnt, st->d_cnt2);
 			} else if (adapt) {
@@ -576,11 +713,24 @@ int tsdrgpu_stack_vectors(tsdrgpu_stack_t *s, int32_t *h_v, int ntiles) {
 	tsdrgpu_ctx_t *ctx = s->ctx;
 	BIND(ctx);
 	const StackState &st = s->st;
-	ARG_TRY(ctx, h_v && st.mode == TSDRGPU_STACK_TRACK && st.m > 0 && st.d_track.ptr);
+	ARG_TRY(ctx, h_v && (st.mode == TSDRGPU_STACK_TRACK || st.mode == TSDRGPU_STACK_ROBUST) && st.m > 0 && st.d_track.ptr);
 	ARG_TRY(ctx, (size_t) ntiles == st_tiles_x(st.w) * st_tiles_y(st.h));
 	CU_TRY(ctx, cudaDeviceSynchronize());
 	CU_TRY(ctx, cudaMemcpy2D(h_v, 2 * sizeof(int32_t), &st.d_track.ptr[0].bx, sizeof(StackTrack), 2 * sizeof(int32_t), (size_t) ntiles,
 	                         cudaMemcpyDeviceToHost));
+	return TSDRGPU_OK;
+}
+
+int tsdrgpu_stack_robust_counts(tsdrgpu_stack_t *s, int32_t *held_tiles, uint64_t *gated_pixels, int32_t *frame_held) {
+	ARG_TRY((tsdrgpu_ctx_t *) NULL, s != NULL);
+	tsdrgpu_ctx_t *ctx = s->ctx;
+	BIND(ctx);
+	const StackState &st = s->st;
+	ARG_TRY(ctx, held_tiles && gated_pixels && frame_held && st.mode == TSDRGPU_STACK_ROBUST && st.m > 0 && st.d_rframe.ptr);
+	StackRobustFrame fr;
+	CU_TRY(ctx, cudaDeviceSynchronize());
+	CU_TRY(ctx, cudaMemcpy(&fr, st.d_rframe.ptr, sizeof fr, cudaMemcpyDeviceToHost));
+	*held_tiles = fr.held; *gated_pixels = fr.gated; *frame_held = fr.hold;
 	return TSDRGPU_OK;
 }
 

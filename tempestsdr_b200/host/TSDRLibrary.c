@@ -418,14 +418,15 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 			goto end;
 		}
 	}
-	/* TSDR_STACK=align:<N>[:<rx>x<ry>], adapt:<N>[:<rx>x<ry>] or track:<N>[:<rx>x<ry>]: drift-registered averaging of the
-	 * delivered frames, ahead of NLM and CLAHE, adapt restarting it tile by tile where the picture changes, track carrying each
-	 * tile's average with content that moves (tsdrgpu.h).  Unset or "off": none */
+	/* TSDR_STACK=align:<N>[:<rx>x<ry>], adapt:<N>[:<rx>x<ry>], track:<N>[:<rx>x<ry>] or robust:<N>[:<rx>x<ry>]: drift-registered
+	 * averaging of the delivered frames, ahead of NLM and CLAHE, adapt restarting it tile by tile where the picture changes, track
+	 * carrying each tile's average with content that moves, robust as track ignoring disturbances that last one frame
+	 * (tsdrgpu.h).  Unset or "off": none */
 	int st_mode = TSDRGPU_STACK_OFF, st_depth = 0, st_rx = 0, st_ry = 0;
 	{
 		const char *st = getenv("TSDR_STACK");
 		if (st && tsdrgpu_stack_parse(st, &st_mode, &st_depth, &st_rx, &st_ry) != TSDRGPU_OK) {
-			status = fail(t, "TSDR_STACK must be \"off\", \"align:<N>[:<rx>x<ry>]\", \"adapt:<N>[:<rx>x<ry>]\" or \"track:<N>[:<rx>x<ry>]\" with N in [2, 1024], rx in [1, 32] and ry in [0, 8]",
+			status = fail(t, "TSDR_STACK must be \"off\", \"align:<N>[:<rx>x<ry>]\", \"adapt:<N>[:<rx>x<ry>]\", \"track:<N>[:<rx>x<ry>]\" or \"robust:<N>[:<rx>x<ry>]\" with N in [2, 1024], rx in [1, 32] and ry in [0, 8]",
 			              TSDR_INVALID_PARAMETER_VALUE);
 			goto end;
 		}

@@ -153,8 +153,8 @@ class Pipeline:
     def set_stack(self, spec: str) -> None:
         """"off" (the default), "align:<N>[:<rx>x<ry>]" (drift-registered averaging of the delivered frames, ahead of NLM and
         CLAHE, tsdrgpu.h), "adapt:<N>[:<rx>x<ry>]" (the same, restarting tile by tile where the picture changes) or
-        "track:<N>[:<rx>x<ry>]" (the same, carrying each tile's average with content that scrolls or moves) from the next
-        frame-stage batch on.  While it is on, on_value also receives (101, drift in px/frame,
+        "track:<N>[:<rx>x<ry>]" (the same, carrying each tile's average with content that scrolls or moves) or
+        "robust:<N>[:<rx>x<ry>]" (track, ignoring disturbances that last one frame) from the next frame-stage batch on.  While it is on, on_value also receives (101, drift in px/frame,
         offset mod W H) beside every auto-gain report; sync() restarts the average."""
         N.check(self._lib.tsdrgpu_pipeline_set_stack(self._h, *N.stack_mode(spec)), self._ctx)
 
