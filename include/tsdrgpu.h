@@ -849,6 +849,72 @@ TSDRGPU_API int  tsdrgpu_superb_mgpu_stitch(tsdrgpu_superb_mgpu_t *g, void *stre
 TSDRGPU_API int  tsdrgpu_superb_mgpu_stream_window(tsdrgpu_superb_mgpu_t *g, float **d_stream);
 TSDRGPU_API int  tsdrgpu_superb_mgpu_lags(tsdrgpu_superb_mgpu_t *g, void *stream, int *h_lags, uint32_t *h_status);
 
+/* ---------------------------------------------------------------------------- a22+  coherent superbandwidth (beyond the reference)
+ * The reference's mode above records hop 0 wherever the front end was left (two of its four hops share a tuning), copies each
+ * hop's spectrum in FFT order to bins that have nothing to do with its tuning, and aligns the hops by an integer lag only.  The
+ * coherent mode records H hops at known, overlapping tunings, places each hop's bins at their true frequencies, and matches
+ * every hop to its neighbour in delay (to 1/1024 sample), phase and gain over their common bins.  It assumes the screen shows
+ * the same picture over the whole round (as the reference's own alignment does): the joins are fitted on that common content.
+ *
+ * Spec (tsdrgpu_superband_t).  mode TSDRGPU_SUPERBAND_REFERENCE (0, the default): the reference's path, unchanged.  mode
+ *   TSDRGPU_SUPERBAND_COHERENT (1): H = hops in {2, 4, 8}, overlap o = overlap_pct in [10, 50] percent.
+ * Schedule (tsdrgpu_superband_schedule).  N = fft_getrealsize(10 floor(fs / fv)) pairs of each hop are used (the reference's
+ *   10 frames).  Hop spacing D = 2 round((1 - o/100) N/2) bins (even; round half away from zero), overlap M = N - D.  Hop i is
+ *   centred at c_i = (i - (H-1)/2) D bins of the stitched band and recorded at offset round(c_i fs / N) Hz through the retune
+ *   callback.  Every hop, hop 0 included, is recorded after a retune and the 0.5 s pause.  A drop restarts the hop in progress.
+ * Stitch (tsdrgpu_superb_stitch_coherent), with centred bin indices.  Hop r = floor((H-1)/2) is the reference; the joins chain
+ *   outward from it (r+1, ..., H-1, then r-1, ..., 0): each newly placed hop b is matched to its corrected neighbour a.
+ *   1. X_i = FFT_N(hop_i) / N (float32, exact stage angles).  Stitched bin kappa of hop i is its bin k = kappa - c_i.
+ *   2. Overlap of a and b: M bins from kappa0 = c_upper - N/2, m = 0 .. M-1.  A_m, B_m the two hops' bins there (A corrected),
+ *      C_m = A_m conj(B_m), u_m = sin^2 theta_m cos^2 theta_m, theta_m = pi (m + 1/2) / M (the crossfade weights' product).
+ *   3. S(tau) = sum_m u_m C_m e^{2 pi i m tau / N}, in double.  tau0 = the first maximum of |S| over integers, from the N-point
+ *      inverse transform of u C and the first-max argmax, mapped to (-N/2, N/2].  tau1 = the best of tau0 + j/32, tau^ the best of
+ *      tau1 + j/1024 (j = -32 .. 32, S evaluated directly, ties to the smallest j).  g = S(tau^) / sum u |B|^2;
+ *      rho = |S(tau^)| / sqrt(sum u |A|^2 sum u |B|^2) in [0, 1].  If sum u |B|^2 = 0: g = 0, tau^ = 0, rho = 0.
+ *   4. B'_kappa = g B_kappa e^{-2 pi i (kappa - kappa0) tau^ / N} for every bin of hop b (a delay is a ramp over the whole band).
+ *   5. Y over L = H N bins: in an overlap the lower hop weighs cos^2 theta_m, the upper sin^2 theta_m, elsewhere in a hop's band
+ *      1; bins no hop covers are 0.  The hops span N + (H-1) D <= L bins, centred.
+ *   6. y = IFFT_L(Y), unscaled (a tone of amplitude A in a hop keeps amplitude A): L pairs at H fs.
+ *   Phases are formed in double from integers reduced mod 1 before sincospi (tau^ = T / 1024 with T an integer); every sum is in
+ *   double with a fixed order (no atomics): the same inputs give the same bits.  The pipeline hands y to the decimator at H fs
+ *   as the one-GPU reference path does. */
+enum { TSDRGPU_SUPERBAND_REFERENCE = 0, TSDRGPU_SUPERBAND_COHERENT = 1 };
+#define TSDRGPU_SUPERBAND_DEFAULT_HOPS    4
+#define TSDRGPU_SUPERBAND_DEFAULT_OVERLAP 25
+#define TSDRGPU_SUPERBAND_MIN_OVERLAP     10
+#define TSDRGPU_SUPERBAND_MAX_OVERLAP     50
+#define TSDRGPU_SUPERBAND_MAX_HOPS        8
+typedef struct {
+	int32_t mode;                                    /* TSDRGPU_SUPERBAND_* */
+	int32_t hops;                                    /* H (coherent) */
+	int32_t overlap_pct;                             /* o (coherent) */
+} tsdrgpu_superband_t;
+/* one join of a coherent stitch (48 bytes) */
+typedef struct {
+	int32_t hop, neighbour;                          /* b, a */
+	int32_t tau0;                                    /* integer lag, in (-N/2, N/2] */
+	int32_t kappa0;                                  /* lowest stitched bin of the overlap */
+	int64_t tau_1024;                                /* tau^ x 1024, exact */
+	double  tau;                                     /* tau^ in samples at fs */
+	double  g_re, g_im;                              /* g */
+	double  rho;                                     /* join quality, 0 .. 1 */
+} tsdrgpu_superband_est_t;
+/* host-only: the spelling shared by the host library's TSDR_SUPERBAND and Python.  "reference", or "coherent[:<H>[:<o>]]" (default
+ * coherent:4:25); H and o are one to six decimal digits in the ranges above, nothing else.  TSDRGPU_OK with *out set, else
+ * TSDRGPU_EINVAL and *out untouched. */
+TSDRGPU_API int  tsdrgpu_superband_parse(const char *spec, tsdrgpu_superband_t *out);
+/* host-only: the schedule of a coherent spec at fs > 0 and refresh rate fv > 0: *n = N, *d = D and offsets[i] (H values, may be
+ * NULL) the retune offsets in Hz.  TSDRGPU_EINVAL for a spec that is not coherent and valid, N < 16, 10 floor(fs / fv) beyond 32 bits, or
+ * an offset outside int32 (which no fs up to the host library's 500 MS/s reaches: |offset| <= 3.15 fs). */
+TSDRGPU_API int  tsdrgpu_superband_schedule(const tsdrgpu_superband_t *spec, uint32_t fs, double refreshrate, uint32_t *n, uint32_t *d,
+                                            int32_t *offsets);
+/* asynchronous, never synchronises the host: the coherent stitch of `nhops` hops (d_hops: device pointers in a HOST array, each at
+ * least count_pairs pairs) with hop spacing d (even, N/2 <= d < N, N = fft_getrealsize(count_pairs)).  d_out receives L = nhops N
+ * interleaved pairs; d_est (device memory) nhops - 1 records, that of hop b at index b - (b > r).  Work memory is the context's
+ * scratch: once a call of a size has run, the next call of that size allocates nothing. */
+TSDRGPU_API int  tsdrgpu_superb_stitch_coherent(tsdrgpu_ctx_t *ctx, void *stream, float *const *d_hops, int nhops, int count_pairs, int d,
+                                                float *d_out, tsdrgpu_superband_est_t *d_est);
+
 /* ---------------------------------------------------------------------------- a1, a3, a5, a16, a17  streaming pipeline
  * replaces the body of process() (TSDRLibrary.c:264-298), decimatingthread / postprocessingthread /
  * videodecodingthread (TSDRLibrary.c:300-418) with their three rings (circbuff.c), dsp_dropped_compensation_*
@@ -919,6 +985,13 @@ TSDRGPU_API int  tsdrgpu_pipeline_set_retune(tsdrgpu_pipeline_t *p, tsdrgpu_retu
  * devices of this node with peer access; hop i is recorded into device i's memory and transformed there, device 0 receives the
  * stitched magnitude stream and makes the frames.  n <= 1: back to 4 hops on one GPU (the reference's SUPER_HOPS_TO_MAKE). */
 TSDRGPU_API int  tsdrgpu_pipeline_set_superb_devices(tsdrgpu_pipeline_t *p, const int *devices, int n);
+/* superbandwidth stitch (see tsdrgpu_superb_stitch_coherent; NULL: TSDRGPU_SUPERBAND_REFERENCE, the default), taking effect at the
+ * next round.  The coherent mode runs on one GPU: a coherent spec while set_superb_devices holds n > 1 devices is refused with
+ * TSDRGPU_EINVAL, and so is set_superb_devices with n > 1 while the spec is coherent. */
+TSDRGPU_API int  tsdrgpu_pipeline_set_superband(tsdrgpu_pipeline_t *p, const tsdrgpu_superband_t *spec);
+/* the last coherent round's joins (synchronises): *n = H - 1 records into out (capacity cap), in tsdrgpu_superb_stitch_coherent's
+ * order; *n = 0 before the first coherent stitch.  Call it between process() calls. */
+TSDRGPU_API int  tsdrgpu_pipeline_superband_estimates(tsdrgpu_pipeline_t *p, tsdrgpu_superband_est_t *out, int cap, int *n);
 /* Page-lock the caller's sample buffers in place (cudaHostRegister) once the same buffer has been handed to process() three
  * times, so that pageable plugin memory crosses PCIe by direct DMA.  Off by default: only for callers that keep their buffer
  * mapped for the whole run (the reference's plugins malloc once per tsdrplugin_readasync); released at destroy. */

@@ -163,6 +163,38 @@ def stack_mode(spec: str):
     return tuple(o.value for o in out)
 
 
+SUPERBAND_REFERENCE, SUPERBAND_COHERENT = 0, 1          # TSDRGPU_SUPERBAND_REFERENCE / _COHERENT
+
+
+class SuperbandSpec(C.Structure):
+    """tsdrgpu_superband_t"""
+    _fields_ = [("mode", C.c_int32), ("hops", C.c_int32), ("overlap_pct", C.c_int32)]
+
+
+class SuperbandEst(C.Structure):
+    """tsdrgpu_superband_est_t: one join of a coherent stitch"""
+    _fields_ = [("hop", C.c_int32), ("neighbour", C.c_int32), ("tau0", C.c_int32), ("kappa0", C.c_int32), ("tau_1024", C.c_int64),
+                ("tau", C.c_double), ("g_re", C.c_double), ("g_im", C.c_double), ("rho", C.c_double)]
+
+
+def superband_spec(spec: str) -> SuperbandSpec:
+    """"reference" or "coherent[:<H>[:<o>]]" (the host library's TSDR_SUPERBAND spelling), read by tsdrgpu_superband_parse."""
+    out = SuperbandSpec()
+    if lib().tsdrgpu_superband_parse(spec.encode(), C.byref(out)) != 0:
+        raise ValueError(f"superband must be 'reference' or 'coherent[:<H>[:<o>]]' with H in {{2, 4, 8}} and o in [10, 50], not {spec!r}")
+    return out
+
+
+def superband_schedule(spec: str, samplerate: int, refreshrate: float):
+    """(N, D, retune offsets in Hz) of a coherent spec, from tsdrgpu_superband_schedule."""
+    s = superband_spec(spec)
+    n, d = C.c_uint32(0), C.c_uint32(0)
+    offs = (C.c_int32 * max(s.hops, 1))()
+    if lib().tsdrgpu_superband_schedule(C.byref(s), samplerate, refreshrate, C.byref(n), C.byref(d), offs) != 0:
+        raise ValueError(f"no coherent superbandwidth schedule for {spec!r} at {samplerate} S/s and {refreshrate} Hz")
+    return n.value, d.value, list(offs)
+
+
 _SIGS = {
     "tsdrgpu_device_count": (C.c_int, []),
     "tsdrgpu_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int]),
@@ -308,6 +340,10 @@ _SIGS = {
     "tsdrgpu_superb_mgpu_stitch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_uint32)]),
     "tsdrgpu_superb_mgpu_stream_window": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "tsdrgpu_superb_mgpu_lags": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint32)]),
+    "tsdrgpu_superband_parse": (C.c_int, [C.c_char_p, C.POINTER(SuperbandSpec)]),
+    "tsdrgpu_superband_schedule": (C.c_int, [C.POINTER(SuperbandSpec), C.c_uint32, C.c_double, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                                             C.POINTER(C.c_int32)]),
+    "tsdrgpu_superb_stitch_coherent": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "tsdrgpu_pipeline_create": (C.c_int, [C.c_void_p, C.POINTER(PipelineConfig), FRAME_CB, VALUE_CB, PLOT_CB, C.c_void_p, C.POINTER(C.c_void_p)]),
     "tsdrgpu_pipeline_destroy": (None, [C.c_void_p]),
     "tsdrgpu_pipeline_process": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int64]),
@@ -323,6 +359,8 @@ _SIGS = {
     "tsdrgpu_pipeline_set_motionblur": (C.c_int, [C.c_void_p, C.c_float]),
     "tsdrgpu_pipeline_set_host_registration": (C.c_int, [C.c_void_p, C.c_int]),
     "tsdrgpu_pipeline_set_superb_devices": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),
+    "tsdrgpu_pipeline_set_superband": (C.c_int, [C.c_void_p, C.POINTER(SuperbandSpec)]),
+    "tsdrgpu_pipeline_superband_estimates": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]),
     "tsdrgpu_pipeline_set_reports": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "tsdrgpu_pipeline_set_resampler": (C.c_int, [C.c_void_p, C.c_int]),
     "tsdrgpu_pipeline_set_autogain": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),

@@ -206,6 +206,30 @@ class Context:
         self.chk(self._lib.tsdrgpu_superb_stitch(self._h, self.stream, ptrs, len(hops), pairs, samples_in_frame, out.data_ptr(), offs, C.byref(total)))
         return out[: 2 * total.value], list(offs)
 
+    def superband_stitch_coherent(self, hops: Sequence[torch.Tensor], d: int,
+                                  out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The coherent superbandwidth stitch (tsdrgpu.h, tsdrgpu_superb_stitch_coherent) of H hops with spacing d bins,
+        asynchronous: (H N interleaved pairs, the H - 1 join records as a uint8 tensor on the device, see superband_records)."""
+        pairs = min(h.numel() for h in hops) // 2
+        n = self.fft_getrealsize(pairs)
+        if out is None:
+            out = torch.empty(len(hops) * n * 2, dtype=torch.float32, device=hops[0].device)
+        assert out.dtype == torch.float32 and out.is_cuda and out.is_contiguous() and out.numel() >= 2 * len(hops) * n, \
+            "out must hold 2 H N contiguous float32 values on the device"
+        for t in list(hops) + [out]:
+            assert t.data_ptr() % 8 == 0, "hops and out must be 8-byte aligned (the kernels read and write them as float2)"
+        est = torch.empty((len(hops) - 1) * C.sizeof(N.SuperbandEst), dtype=torch.uint8, device=hops[0].device)
+        ptrs = (C.c_void_p * len(hops))(*[_f32(h).data_ptr() for h in hops])
+        self.chk(self._lib.tsdrgpu_superb_stitch_coherent(self._h, self.stream, ptrs, len(hops), pairs, d, out.data_ptr(), est.data_ptr()))
+        return out, est
+
+    @staticmethod
+    def superband_records(est: torch.Tensor) -> List["N.SuperbandEst"]:
+        """The join records of superband_stitch_coherent's second result (copies them to the host: synchronises)."""
+        raw = est.cpu().numpy().tobytes()
+        k = C.sizeof(N.SuperbandEst)
+        return [N.SuperbandEst.from_buffer_copy(raw[i * k:(i + 1) * k]) for i in range(len(raw) // k)]
+
     # ------------------------------------------------------------------ factories
     def resampler(self) -> "Resampler":
         return Resampler(self)

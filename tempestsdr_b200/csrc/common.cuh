@@ -113,6 +113,8 @@ int tsdrgpu_fft_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, float2 *data, 
 int tsdrgpu_fft_oop_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, unsigned long long n_pow2, int inverse);
 int tsdrgpu_fft_batch_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, long long in_bs, float2 *out, long long out_bs,
                                float2 *scratch, unsigned long long n_pow2, unsigned batch, int inverse);
+int tsdrgpu_fft_exact_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, float2 *scratch, unsigned long long n_pow2,
+                               int inverse);
 bool tsdrgpu_fft_true_dft();          // TSDRGPU_FFT_TRUE_DFT: the exact DFT's stage angles instead of the reference's
 int tsdrgpu_argmax_mag_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *x, unsigned n, void *d_part, int *d_result);
 int fs_copy_async(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float *in, float *out, size_t total);

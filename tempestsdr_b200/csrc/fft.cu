@@ -991,6 +991,15 @@ int tsdrgpu_fft_batch_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const fl
 	o.cplx_in = in; o.cplx_bs = in_bs; o.data_bs = out_bs; o.scratch_bs = (long long) n_pow2;
 	return fft_run(ctx, stream, out, scratch, ilog2(n_pow2), inverse, o);
 }
+// one transform with the exact DFT's stage angles, from `in` (complex, may be `out`) into `out` through `scratch` (n_pow2 complex of
+// the caller's); forward transforms scale by 1/n_pow2, inverse ones are unscaled
+int tsdrgpu_fft_exact_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *in, float2 *out, float2 *scratch, unsigned long long n_pow2,
+                               int inverse) {
+	ARG_TRY(ctx, n_pow2 >= 2);
+	FftOpts o; memset(&o, 0, sizeof o); o.batch = 1; o.scale = inverse ? 1.0f : 1.0f / (float) n_pow2; o.exact = true;
+	if (in != out) { o.cplx_in = in; o.cplx_bs = 0; }
+	return fft_run(ctx, stream, out, scratch, ilog2(n_pow2), inverse, o);
+}
 // *d_result = index of the first maximum of |x[0..n)|; d_part: room for 2 * TSDRGPU_ARGMAX_PARTS 32-bit words
 int tsdrgpu_argmax_mag_internal(tsdrgpu_ctx_t *ctx, cudaStream_t stream, const float2 *x, unsigned n, void *d_part, int *d_result) {
 	unsigned parts = (n + 4095) / 4096; if (parts > TSDRGPU_ARGMAX_PARTS) parts = TSDRGPU_ARGMAX_PARTS; if (parts < 1) parts = 1;

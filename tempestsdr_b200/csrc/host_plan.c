@@ -323,6 +323,49 @@ int tsdrgpu_stack_parse(const char *spec, int *mode, int *depth, int *rx, int *r
 	return TSDRGPU_OK;
 }
 
+/* ---- the coherent superbandwidth mode's spelling and schedule (definitions in tsdrgpu.h) */
+int superband_ok(const tsdrgpu_superband_t *s) {
+	return s->mode == TSDRGPU_SUPERBAND_REFERENCE || (s->mode == TSDRGPU_SUPERBAND_COHERENT && (s->hops == 2 || s->hops == 4 || s->hops == 8) &&
+	       s->overlap_pct >= TSDRGPU_SUPERBAND_MIN_OVERLAP && s->overlap_pct <= TSDRGPU_SUPERBAND_MAX_OVERLAP);
+}
+
+int tsdrgpu_superband_parse(const char *spec, tsdrgpu_superband_t *out) {
+	if (!spec || !out) return TSDRGPU_EINVAL;
+	tsdrgpu_superband_t s = {TSDRGPU_SUPERBAND_REFERENCE, 0, 0};
+	if (strcmp(spec, "reference") != 0) {
+		const char *c = spec;
+		if (strncmp(c, "coherent", 8) != 0) return TSDRGPU_EINVAL;
+		c += 8;
+		s.mode = TSDRGPU_SUPERBAND_COHERENT; s.hops = TSDRGPU_SUPERBAND_DEFAULT_HOPS; s.overlap_pct = TSDRGPU_SUPERBAND_DEFAULT_OVERLAP;
+		if (*c == ':') {
+			c++; if ((s.hops = option_digits(&c)) < 0) return TSDRGPU_EINVAL;
+			if (*c == ':') { c++; if ((s.overlap_pct = option_digits(&c)) < 0) return TSDRGPU_EINVAL; }
+		}
+		if (*c) return TSDRGPU_EINVAL;
+	}
+	if (!superband_ok(&s)) return TSDRGPU_EINVAL;
+	*out = s;
+	return TSDRGPU_OK;
+}
+
+int tsdrgpu_superband_schedule(const tsdrgpu_superband_t *spec, uint32_t fs, double refreshrate, uint32_t *n, uint32_t *d, int32_t *offsets) {
+	if (!spec || !n || !d || !superband_ok(spec) || spec->mode != TSDRGPU_SUPERBAND_COHERENT || fs == 0 || !(refreshrate > 0.0)) return TSDRGPU_EINVAL;
+	const double per_frame = floor((double) fs / refreshrate);
+	if (!(per_frame >= 1.0) || 10.0 * per_frame > 4294967295.0) return TSDRGPU_EINVAL;
+	const uint32_t N = tsdrgpu_fft_getrealsize((uint32_t) (10.0 * per_frame));
+	if (N < 16) return TSDRGPU_EINVAL;
+	const uint32_t D = 2u * (uint32_t) llround((1.0 - spec->overlap_pct / 100.0) * (double) N / 2.0);
+	const int H = spec->hops;
+	for (int i = 0; i < H; i++) {
+		const double c = (double) (2 * i - (H - 1)) * (double) D / 2.0;       /* exact: D is even */
+		const double hz = (double) llround(c * (double) fs / (double) N);
+		if (hz < -2147483648.0 || hz > 2147483647.0) return TSDRGPU_EINVAL;
+		if (offsets) offsets[i] = (int32_t) hz;
+	}
+	*n = N; *d = D;
+	return TSDRGPU_OK;
+}
+
 /* its own small rule, as it takes one optional value: "rl:<sigma>[:<I>]", sigma with at most two fraction digits */
 int tsdrgpu_deblur_parse(const char *spec, int *mode, int *sigma_centi, int *iterations) {
 	if (!spec || !mode || !sigma_centi || !iterations) return TSDRGPU_EINVAL;

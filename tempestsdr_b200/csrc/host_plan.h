@@ -13,6 +13,7 @@ int contrast_ok(int mode, int clip_centi, int tx, int ty);
 int denoise_ok(int mode, int h_milli, int r, int p);
 int stack_ok(int mode, int depth, int rx, int ry);
 int deblur_ok(int mode, int sigma_centi, int iterations);
+int superband_ok(const tsdrgpu_superband_t *s);
 #ifdef __cplusplus
 }
 #endif

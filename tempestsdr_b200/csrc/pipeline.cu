@@ -86,6 +86,7 @@ struct Settings {
 	tsdrgpu_channel_t cf_spec = {};                    // taps == 0: off; applied per process()
 	tsdrgpu_welch_t sp_spec = {};                      // n == 0: off; applied per process()
 	tsdrgpu_coherence_t ch_spec = {};                  // rate == 0: off; applied per process()
+	tsdrgpu_superband_t sbd_spec = {};                 // mode 0: the reference's stitch; latched at the start of each superbandwidth round
 	int host_register = 0;                             // opt-in: tsdrgpu_pipeline_set_host_registration
 	tsdrgpu_retune_cb retune_cb = nullptr;
 };
@@ -234,6 +235,9 @@ struct tsdrgpu_pipeline {
 		// hop i is recorded by rank i; ndev ranks of one hop per GPU (tsdrgpu_pipeline_set_superb_devices), or 0 in the one-GPU mode
 		int ndev; std::unique_ptr<SbRank> rank[16];
 		tsdrgpu_superb_mgpu_t *grp[16];               // the sharded mode's group, one member per rank, once the hop size is known
+		// the round's stitch (Settings::sbd_spec at its start); coherent: the spacing D, the retune offsets, the joins' records
+		tsdrgpu_superband_t spec; uint32_t d; int32_t offsets[TSDRGPU_SUPERBAND_MAX_HOPS];
+		DeviceBuf<tsdrgpu_superband_est_t> d_est; int est_n;
 	} sb;
 	// delivery
 	std::thread thread; std::mutex mu; std::condition_variable cv_job, cv_done;
@@ -759,6 +763,8 @@ int tsdrgpu_pipeline_set_superb_devices(tsdrgpu_pipeline_t *p, const int *device
 	ARG_TRY((tsdrgpu_ctx_t *) NULL, p != NULL);
 	tsdrgpu_ctx_t *ctx = p->ctx;
 	BIND(ctx);
+	if (n > 1 && settings(p).sbd_spec.mode == TSDRGPU_SUPERBAND_COHERENT)
+		return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "the coherent superbandwidth stitch runs on one GPU: set the reference stitch before sharding the hops", cudaSuccess, __FILE__, __LINE__);
 	CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
 	superb_release(p);
 	if (n <= 1) return TSDRGPU_OK;
@@ -766,6 +772,27 @@ int tsdrgpu_pipeline_set_superb_devices(tsdrgpu_pipeline_t *p, const int *device
 	const int rc = superb_ranks(p, devices, n);
 	if (rc) superb_release(p); else p->sb.ndev = n;     // a failure leaves the one-GPU mode, its error text in ctx
 	return rc;
+}
+int tsdrgpu_pipeline_set_superband(tsdrgpu_pipeline_t *p, const tsdrgpu_superband_t *spec) {
+	if (!p) return TSDRGPU_EINVAL;
+	tsdrgpu_superband_t b = {TSDRGPU_SUPERBAND_REFERENCE, 0, 0};
+	if (spec && spec->mode != TSDRGPU_SUPERBAND_REFERENCE) {
+		if (!superband_ok(spec)) return tsdrgpu_fail(p->ctx, TSDRGPU_EINVAL, "invalid superband spec (tsdrgpu.h)", cudaSuccess, __FILE__, __LINE__);
+		if (p->sb.ndev > 1)
+			return tsdrgpu_fail(p->ctx, TSDRGPU_EINVAL, "the coherent superbandwidth stitch runs on one GPU: return to one device (set_superb_devices with n <= 1) first", cudaSuccess, __FILE__, __LINE__);
+		b = *spec;
+	}
+	return update(p, true, [&](Settings &s) { s.sbd_spec = b; });
+}
+int tsdrgpu_pipeline_superband_estimates(tsdrgpu_pipeline_t *p, tsdrgpu_superband_est_t *out, int cap, int *n) {
+	ARG_TRY((tsdrgpu_ctx_t *) NULL, p != NULL && n != NULL);
+	tsdrgpu_ctx_t *ctx = p->ctx;
+	BIND(ctx);
+	ARG_TRY(ctx, p->sb.est_n == 0 || (out != NULL && cap >= p->sb.est_n));
+	CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
+	if (p->sb.est_n) CU_TRY(ctx, cudaMemcpy(out, p->sb.d_est.ptr, sizeof(tsdrgpu_superband_est_t) * p->sb.est_n, cudaMemcpyDeviceToHost));
+	*n = p->sb.est_n;
+	return TSDRGPU_OK;
 }
 int tsdrgpu_pipeline_set_host_registration(tsdrgpu_pipeline_t *p, int on) { return update(p, true, [&](Settings &s) { s.host_register = on != 0; }); }
 int tsdrgpu_pipeline_set_retune(tsdrgpu_pipeline_t *p, tsdrgpu_retune_cb cb) { return update(p, true, [&](Settings &s) { s.retune_cb = cb; }); }
@@ -897,12 +924,26 @@ static int superb_build(tsdrgpu_pipeline *p, const Settings &s, int H, bool shar
 static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq, int fmt, uint64_t items_count, int64_t dropped) {
 	tsdrgpu_ctx_t *ctx = p->ctx;
 	int rc;
-	const bool sharded = p->sb.ndev > 1; const int H = sharded ? p->sb.ndev : 4;       // SUPER_HOPS_TO_MAKE
+	const bool sharded = p->sb.ndev > 1;
 	if (p->sb.state == SB_STOPPED) p->sb.state = SB_STARTING;
+	if (p->sb.state == SB_STARTING) p->sb.spec = s.sbd_spec;                   // a new stitch takes effect at the next round
+	const bool coherent = p->sb.spec.mode == TSDRGPU_SUPERBAND_COHERENT;
+	const int H = coherent ? p->sb.spec.hops : (sharded ? p->sb.ndev : 4);       // SUPER_HOPS_TO_MAKE
 	if (p->sb.state == SB_STARTING) {
 		p->sb.buffid = 0; p->sb.gathered = 0;
-		if ((s.samplerate_real != p->sb.rate || p->sb.nhops != H) && (rc = superb_build(p, s, H, sharded))) { cudaSetDevice(ctx->device); return rc; }
-		p->sb.state = SB_GATHERING;
+		if (coherent && sharded) return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "the coherent superbandwidth stitch runs on one GPU", cudaSuccess, __FILE__, __LINE__);
+		// the coherent mode also follows the hop size when the refresh rate moves it (the reference mode keeps its first one)
+		const bool resize = coherent && (long long) (s.samplerate_real / s.refreshrate) != p->sb.in_frame;
+		if ((s.samplerate_real != p->sb.rate || p->sb.nhops != H || resize) && (rc = superb_build(p, s, H, sharded))) { cudaSetDevice(ctx->device); return rc; }
+		if (coherent) {
+			// every hop, hop 0 included, is recorded after a retune and the pause
+			uint32_t n = 0;
+			if (tsdrgpu_superband_schedule(&p->sb.spec, p->sb.rate, s.refreshrate, &n, &p->sb.d, p->sb.offsets) != TSDRGPU_OK ||
+			    n != tsdrgpu_fft_getrealsize((uint32_t) p->sb.to_gather))
+				return tsdrgpu_fail(ctx, TSDRGPU_EINVAL, "no coherent superbandwidth schedule for this sample rate and refresh rate", cudaSuccess, __FILE__, __LINE__);
+			if (s.retune_cb) s.retune_cb(p->sb.offsets[0], p->user);
+			p->sb.state = SB_PAUSE;
+		} else p->sb.state = SB_GATHERING;
 	}
 	if (p->sb.state == SB_PAUSE) {
 		p->sb.gathered += (long long) (items_count / 2);
@@ -951,7 +992,8 @@ static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq,
 		cudaSetDevice(ctx->device);
 	}
 	if (p->sb.buffid < H) {
-		if (s.retune_cb) s.retune_cb((int32_t) ((p->sb.buffid - H / 2) * (long long) p->sb.rate), p->user);    // shiftfreq, superbandwidth.c:241
+		if (coherent) { if (s.retune_cb) s.retune_cb(p->sb.offsets[p->sb.buffid], p->user); }
+		else if (s.retune_cb) s.retune_cb((int32_t) ((p->sb.buffid - H / 2) * (long long) p->sb.rate), p->user);    // shiftfreq, superbandwidth.c:241
 		p->sb.state = SB_PAUSE;
 		return TSDRGPU_OK;
 	}
@@ -959,7 +1001,25 @@ static int superb_step(tsdrgpu_pipeline *p, const Settings &s, const void *h_iq,
 	const unsigned long long N = tsdrgpu_fft_getrealsize((uint32_t) count_pairs);
 	size_t total_samples = 0;
 	CU_TRY(ctx, cudaStreamSynchronize(p->s_ingest));
-	if (!sharded) {
+	if (coherent) {
+		// the coherent stitch: L = H N pairs at H fs, handed to the decimator as the one-GPU reference path hands its output
+		const size_t L = (size_t) H * N;
+		if (p->sb.d_out.cap < 2 * L || p->sb.d_est.cap < (size_t) H) {
+			CU_TRY(ctx, cudaStreamSynchronize(p->s_main));
+			CU_TRY(ctx, p->sb.d_out.reserve(p->s_main, 2 * L, 0)); CU_TRY(ctx, p->sb.d_est.reserve(p->s_main, (size_t) H, 0));
+		}
+		float *hops[TSDRGPU_SUPERBAND_MAX_HOPS];
+		for (int i = 0; i < H; i++) hops[i] = p->sb.rank[i]->hop.ptr;
+		if ((rc = tsdrgpu_superb_stitch_coherent(ctx, p->s_main, hops, H, (int) count_pairs, (int) p->sb.d, p->sb.d_out.ptr, p->sb.d_est.ptr))) return rc;
+		p->sb.est_n = H - 1;
+		CU_TRY(ctx, cudaEventRecord(p->sb.ev, p->s_main));
+		float *where;
+		if ((rc = decim_set_elem(p, 2))) return rc;
+		if ((rc = decim_reserve(p, L, &where))) return rc;
+		pl_copy_f32<<<2048, 256, 0, p->s_main>>>(p->sb.d_out.ptr, where, 2 * L);
+		LAUNCH_CHECK(ctx);
+		total_samples = L;
+	} else if (!sharded) {
 		if (p->sb.d_out.cap < 2 * (size_t) H * N) { CU_TRY(ctx, cudaStreamSynchronize(p->s_main)); CU_TRY(ctx, p->sb.d_out.assign(2 * (size_t) H * N)); }
 		int offs[16], total = 0;
 		float *hops[16];

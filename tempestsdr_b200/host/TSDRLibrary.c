@@ -443,6 +443,17 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 		}
 	}
 
+	/* TSDR_SUPERBAND=coherent[:<H>[:<o>]]: superbandwidth mode records H overlapping hops at their true frequencies and stitches them
+	 * with matched delay, phase and gain (tsdrgpu.h).  Unset or "reference": the reference's stitch */
+	tsdrgpu_superband_t superband = {TSDRGPU_SUPERBAND_REFERENCE, 0, 0};
+	{
+		const char *sb = getenv("TSDR_SUPERBAND");
+		if (sb && tsdrgpu_superband_parse(sb, &superband) != TSDRGPU_OK) {
+			status = fail(t, "TSDR_SUPERBAND must be \"reference\" or \"coherent[:<H>[:<o>]]\" with H in {2, 4, 8} and o in [10, 50]", TSDR_INVALID_PARAMETER_VALUE);
+			goto end;
+		}
+	}
+
 	/* TSDR_CUDA_DEVICES="0,1,2,3": superbandwidth mode records one hop per listed GPU and shards the stitch over them
 	 * (tsdrgpu_pipeline_set_superb_devices); the first entry is the device everything else runs on.  TSDR_CUDA_DEVICE=n: one GPU. */
 	int devlist[16], ndev = 0;
@@ -480,7 +491,8 @@ int tsdr_readasync(tsdr_lib_t *t, tsdr_readasync_function cb, void *ctx) {
 		tsdrgpu_pipeline_set_retune(np, on_retune);
 		/* a plugin keeps its buffer for the whole tsdrplugin_readasync (TSDRPlugin_RawFile.c:212, 263): page-lock it in place */
 		tsdrgpu_pipeline_set_host_registration(np, getenv("TSDR_NO_HOST_REGISTER") ? 0 : 1);
-		if (ndev > 1 && tsdrgpu_pipeline_set_superb_devices(np, devlist, ndev) != TSDRGPU_OK) {
+		if ((ndev > 1 && tsdrgpu_pipeline_set_superb_devices(np, devlist, ndev) != TSDRGPU_OK) ||
+		    (superband.mode != TSDRGPU_SUPERBAND_REFERENCE && tsdrgpu_pipeline_set_superband(np, &superband) != TSDRGPU_OK)) {
 			status = fail(t, tsdrgpu_last_error(t->gpu), TSDR_CANNOT_OPEN_DEVICE);
 			tsdrgpu_pipeline_destroy(np);
 			goto end;

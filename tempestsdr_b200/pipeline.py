@@ -26,7 +26,7 @@ class Pipeline:
                  on_frame: Optional[Callable] = None, on_value: Optional[Callable] = None, on_plot: Optional[Callable] = None,
                  on_retune: Optional[Callable] = None, resampler: str = "box", autogain: str = "minmax",
                  contrast: str = "off", channel: str = "off", denoise: str = "off", spectrum: str = "off",
-                 stack: str = "off", deblur: str = "off", coherence: str = "off"):
+                 stack: str = "off", deblur: str = "off", coherence: str = "off", superband: str = "reference"):
         self._lib = N.lib()
         ctx = C.c_void_p()
         N.check(self._lib.tsdrgpu_create(C.byref(ctx), device))
@@ -81,6 +81,8 @@ class Pipeline:
             self.set_stack(stack)
         if deblur != "off":
             self.set_deblur(deblur)
+        if superband != "reference":
+            self.set_superband(superband)
         if on_retune:
             def _retune(off, _):
                 try:
@@ -189,6 +191,18 @@ class Pipeline:
         """Superbandwidth mode with one hop per GPU: devices[0] is this pipeline's device, len(devices) in {2, 4, 8} = hops."""
         arr = (C.c_int * len(devices))(*devices)
         N.check(self._lib.tsdrgpu_pipeline_set_superb_devices(self._h, arr, len(devices)), self._ctx)
+
+    def set_superband(self, spec: str) -> None:
+        """"reference" (the reference's stitch, the default) or "coherent[:<H>[:<o>]]" (H overlapping hops at their true
+        frequencies, matched in delay, phase and gain, tsdrgpu.h) from the next superbandwidth round on.  One GPU only."""
+        N.check(self._lib.tsdrgpu_pipeline_set_superband(self._h, C.byref(N.superband_spec(spec))), self._ctx)
+
+    def superband_estimates(self):
+        """The last coherent round's joins (tsdrgpu_superband_est_t records, one per hop but the reference hop); synchronises."""
+        recs = (N.SuperbandEst * 8)()
+        n = C.c_int(0)
+        N.check(self._lib.tsdrgpu_pipeline_superband_estimates(self._h, recs, 8, C.byref(n)), self._ctx)
+        return list(recs[: n.value])
 
     def set_motionblur(self, coeff: float) -> None:
         N.check(self._lib.tsdrgpu_pipeline_set_motionblur(self._h, coeff), self._ctx)
